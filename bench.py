@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rays/sec of the SceneRF ray-render hot path on B200 (BASELINE.json metric), one JSON line.
+"""bench.py -- rays/sec of the SceneRF ray-render hot path on one H100 (BASELINE.json metric), one JSON line.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload B|A|C] [--precision fp16|fp32]
 
@@ -165,10 +165,9 @@ def cpu_port_rays_per_sec(cfg, pix, pyramid, target_seconds=15.0, chunk=128):
                                     % (n_rays, cfg.S, chunk, workers, blas, dt))
 
 
-# Fixed layout of the reference CPU arm, chosen by tools/ref_probe.py on the B200 box's host (2 x 32-core Xeon 8562Y+,
-# 128 logical CPUs; profiles/r2_reference_cpu_layout_probe.log): ONE process with 64-128 intra-op threads reaches only
-# 35-300 rays/s (the reference's chain of small ops does not scale past ~16 threads), 8 processes x 16 threads reach
-# 800-950 rays/s.  So the arm is 8 worker processes, each running the reference's own class on its own rays.
+# Fixed layout of the reference CPU arm (tools/ref_probe.py compares layouts): the reference's chain of small ops does
+# not scale past ~16 intra-op threads in one process, so the arm is 8 worker processes, each running the reference's own
+# class on its own rays.
 REF_PROCS = 8
 REF_RAYS_PER_PROC = 512          # rays per reference call (one chunk): 8 x 512 = 4096 rays per step
 
@@ -333,7 +332,7 @@ def run_reference(args, rank, world):
                "cpus": pool.cpu_info,
                "sample": "each step = %d concurrent calls (one per process, %d torch threads each) of the reference's SceneRF.render_rays_batch "
                          "(unmodified sources in oracle/_ref through the SURVEY 8c shim) on %d random rays x %d samples of the workload in one chunk; "
-                         "step times min/median/max %.2f/%.2f/%.2f s; layout fixed by profiles/r2_reference_cpu_layout_probe.log"
+                         "step times min/median/max %.2f/%.2f/%.2f s; process layout compared by tools/ref_probe.py"
                          % (pool.procs, pool.threads, n, cfg.S, min(times), float(np.median(times)), max(times))}
         what = "the reference's own SceneRF class (unmodified sources staged in oracle/_ref) on host cores"
         rays_per_step = n * pool.procs
@@ -530,7 +529,7 @@ def run_train(args, rank, world, local):
     fwd_ms, bwd_ms = e[2].elapsed_time(e[3]), e[3].elapsed_time(e[0])
     flop_fwd = R * flop_per_ray(cfg)
     flop_step = 4.0 * flop_fwd          # forward + recompute + dX GEMMs + dW GEMMs, each = one forward's FLOPs
-    fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12          # 148 SMs x 128 FMA lanes x 2 x max clock
+    fp32_peak = H100_FP32_TFLOPS                        # 132 SMs x 128 FMA lanes x 2 x 1.98 GHz (data sheet)
     bound = "fp32 FMA (SIMT)"
     if args.train_matmul == "tf32":
         peaks = {}
@@ -538,8 +537,8 @@ def run_train(args, rank, world, local):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        fp32_peak = float(peaks.get("bf16_tflops_sustained") or 1400.0) / 2.0      # kind::tf32 issues at half the kind::f16 rate
-        bound = "tensor (tcgen05 kind::tf32; peak = measured bf16 sustained / 2)"
+        fp32_peak = float(peaks.get("bf16_tflops_sustained") or H100_FP16_TFLOPS) / 2.0      # wgmma tf32 issues at half the f16 rate
+        bound = "tensor (wgmma tf32; peak = fp16 peak / 2)"
     res = {"metric": "training rays/sec (render_rays_batch forward + backward, %d rays x %d samples per step)" % (R, cfg.S),
            "value": world * R / (ms * 1e-3), "unit": "rays/s", "ms_per_step": ms, "n_gpus": world, "steps": args.steps,
            "warmup": args.warmup, "dtype": "f32" if args.train_matmul == "fp32" else "tf32 operands, f32 storage and accumulate",
@@ -549,10 +548,10 @@ def run_train(args, rank, world, local):
            "roofline": {"bound": bound, "achieved": 3.0 * flop_fwd / (ms * 1e-3) / 1e12, "peak": fp32_peak, "unit": "TFLOP/s",
                         "frac": 3.0 * flop_fwd / (ms * 1e-3) / 1e12 / fp32_peak,
                         "algorithmic_flop_per_step": 3.0 * flop_fwd, "dense_flop_per_step_with_recompute": flop_step,
-                        "note": "ALGORITHMIC flops (forward + dX + dW of the dense 2480-wide latent) / time; SIMT peak = 148 SMs x 128 lanes x "
-                                "2 FLOP x 1.965 GHz.  Not a utilisation figure: the lin_z K-segments of pyramid scales that no point of a "
-                                "chunk reaches (exact zeros, quirk Q2; typically 2240 of the 2480 latent columns) are skipped on the "
-                                "device, and the backward recomputes the forward per 9472-point chunk"}}
+                        "note": "ALGORITHMIC flops (forward + dX + dW of the dense 2480-wide latent) / time; SIMT peak = 132 SMs x 128 lanes x "
+                                "2 FLOP x 1.98 GHz (data sheet).  Not a utilisation figure: the lin_z K-segments of pyramid scales that no point of a "
+                                "pass reaches (exact zeros, quirk Q2; typically 2240 of the 2480 latent columns) are skipped on the "
+                                "device; dense_flop_per_step_with_recompute also counts a recomputed forward"}}
     if rank == 0 and not args.no_cpu_baseline:
         from oracle import scenerf_oracle as so, backward_oracle as bo
         n = 24
@@ -613,7 +612,7 @@ def run_lattice(args, rank, world, local):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("bf16_tflops_sustained") or 1400.0)
+    peak = float(peaks.get("bf16_tflops_sustained") or H100_FP16_TFLOPS)
     res = {"metric": "lattice points/sec (density query of the 256^3 lattice)", "value": n_pts / (ms * 1e-3), "unit": "points/s",
            "ms_per_step": ms, "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "dtype": args.precision, "data": "synthetic",
            "scaling": "strong", "higher_is_better": True, "gpu_launches": int(r.last_lattice_launches),
@@ -640,6 +639,11 @@ def run_lattice(args, rank, world, local):
         dist.destroy_process_group()
 
 
+# NVIDIA H100 SXM data sheet (700 W card), dense: fallbacks for the rooflines when no measured peak is on the machine
+H100_FP16_TFLOPS = 989.0
+H100_FP32_TFLOPS = 67.0
+
+
 def load_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
@@ -647,8 +651,8 @@ def load_peaks():
         return {}
 
 
-PREC_DESC = {"fp32tc": "fp32-grade on tensor cores: fp16 hi/lo split operands (22 mantissa bits), fp32 accumulate in TMEM (tcgen05 kind::f16, 4 partial products)",
-             "fp16": "fp16 operands, fp32 accumulate (tcgen05 kind::f16) -- reduced-precision fast mode",
+PREC_DESC = {"fp32tc": "fp32-grade on tensor cores: fp16 hi/lo split operands (22 mantissa bits), fp32 accumulate (wgmma f16, 4 partial products)",
+             "fp16": "fp16 operands, fp32 accumulate (wgmma f16) -- reduced-precision fast mode",
              "fp32": "fp32 SIMT FMA"}
 PREC_DTYPE = {"fp32tc": "fp32 (2 x fp16 split operands, fp32 accumulate)", "fp16": "fp16", "fp32": "f32"}
 
@@ -766,6 +770,28 @@ def measure_workload_E(args, rank, world, dev, sync, r, x_rgb, cfg):
             "tflops_algorithmic": n_pts * FLOP_MAIN / (ms * 1e-3) / 1e12, "gpu_launches": int(r.last_lattice_launches)}
 
 
+def dump_outputs(out_dir, outs, budget=64 << 20):
+    """--dump-outputs: every array the timed call returned in its last step, as out_dir/<name>.npy (float32; float64
+    stays float64).  When they would exceed `budget` bytes together, the same fixed, seeded sample of rays (rows) is kept
+    of every per-ray array and its row numbers are written as ray_index.npy."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrs = {}
+    for k, v in outs.items():
+        if torch.is_tensor(v):
+            v = v.detach()
+            arrs[k] = (v if v.dtype == torch.float64 else v.float()).cpu().numpy()
+    n_rows = max((a.shape[0] for a in arrs.values() if a.ndim), default=0)
+    total = sum(a.nbytes for a in arrs.values())
+    if total > budget and n_rows > 0:
+        keep = max(1, int(n_rows * budget / total))
+        idx = np.sort(np.random.default_rng(0).choice(n_rows, keep, replace=False))
+        arrs = {k: (a[idx] if a.ndim and a.shape[0] == n_rows else a) for k, a in arrs.items()}
+        arrs["ray_index"] = idx.astype(np.float64)
+    for k, a in arrs.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.ascontiguousarray(a))
+
+
 def run_render(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -822,8 +848,9 @@ def run_render(args, rank, world, local_rank):
     mlp_ms = []
     launches = 0
     ev0.record()
+    last = None
     for _ in range(args.steps):
-        step_device()
+        last = step_device()
         launches += r.last_launches
         mlp_ms.append(r.last_mlp_ms()[1])            # waits for this step's main-MLP end event only
     ev1.record()
@@ -831,6 +858,8 @@ def run_render(args, rank, world, local_rank):
     clocks = sampler.stop()
     ms_per_step = max_over_ranks(ev0.elapsed_time(ev1), dev, world) / args.steps
     value = world * R / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last if isinstance(last, dict) else dict(zip(("depth", "color"), last)))
 
     # ---- e2e: host buffers in, host buffers out, through the reference-facing call ------------------------------
     out_host = {"depth": torch.empty((R,), dtype=torch.float32).pin_memory(),
@@ -877,29 +906,21 @@ def run_render(args, rank, world, local_rank):
 
     # ---- roofline of the dominant kernel (main point-MLP pass), measured live with CUDA events ------------------
     peaks = load_peaks()
-    peak = peaks.get("bf16_tflops_sustained") or 1400.0
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (fp16 and bf16 share the tcgen05 kind::f16 rate; the kernel runs inside a seconds-long step)" \
-        if peaks else "fallback 1.4 PF sustained (B200_PROFILING.md)"
+    peak = peaks.get("bf16_tflops_sustained") or H100_FP16_TFLOPS
+    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (fp16 and bf16 share the wgmma f16 rate; the kernel runs inside a seconds-long step)" \
+        if peaks else "H100 SXM data-sheet dense fp16 rate (700 W card), not a measured rate"
     main_ms = float(np.mean([m for m in mlp_ms if m > 0])) if mlp_ms else float("nan")
     flop_launch = float(R) * cfg.S * FLOP_MAIN
     achieved = flop_launch / (main_ms * 1e-3) / 1e12
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(args.workload + "_" + args.precision)
-    except Exception:
-        pass
     mma_mult = 4.0 if args.precision == "fp32tc" else 1.0
     roofline = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_unit": "DRAM bytes per launch (ncu dram__bytes_read.sum + dram__bytes_write.sum, profiles/traffic.json)",
                 "kernel": "point_mlp_tc_kernel (main pass)" if args.precision != "fp32" else "sgemm_nt_kernel chain",
                 "kernel_ms": main_ms, "algorithmic_flop_per_launch": flop_launch, "peak_source": peak_src,
                 "executed_tensor_tflops": achieved * mma_mult * 1.025, "executed_frac": achieved * mma_mult * 1.025 / peak,
                 "peak_burst": peaks.get("bf16_tflops"), "executed_frac_of_burst": (achieved * mma_mult * 1.025 / peaks["bf16_tflops"]) if peaks.get("bf16_tflops") else None,
                 "note": "achieved = ALGORITHMIC flops (10 811 392 per sample point) / kernel time, per GPU (rank 0's launch). " +
                         ("fp32tc issues 4 fp16 MMAs per algorithmic product, (x_hi,x_lo) x (W_hi,W_lo): executed_* = 4 x 1.025 (K/N padding) x algorithmic, "
-                         "i.e. frac can reach 0.25 of the kind::f16 rate at most; executed_frac is the tensor-pipe figure.  It can exceed 1 against the "
-                         "SUSTAINED peak: cuBLAS sustains 1456 TFLOP/s at ~1.4 GHz under the 1 kW cap while this kernel holds ~1.65 GHz "
-                         "(clocks in this line); executed_frac_of_burst is against the 1709 TFLOP/s burst figure" if args.precision == "fp32tc"
+                         "i.e. frac can reach 0.25 of the f16 rate at most; executed_frac is the tensor-pipe figure" if args.precision == "fp32tc"
                          else "executed = 1.025 x algorithmic (K padded 42->64, 2480->2496, N 4->16)"),
                 "whole_step_tflops_per_gpu": R * flop_per_ray(cfg) / (ms_per_step * 1e-3) / 1e12}
 
@@ -1033,11 +1054,15 @@ def main():
     ap.add_argument("--latent-table", type=int, default=0, help="1: the timed renderer uses the pre-projected latent table (diagnostics / profiling)")
     ap.add_argument("--no-extras", action="store_true", help="skip the strong-scaling / workload D / workload E measurements")
     ap.add_argument("--e2e-steps", type=int, default=0, help="steps of the host-buffer (e2e) loop; 0 = same as --steps")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the arrays the timed call returned in its last step as DIR/<name>.npy (render workloads A, B, Bp, C)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.dump_outputs and (args.impl != "ours" or args.workload not in ("A", "B", "Bp", "C")):
+        ap.error("--dump-outputs applies to the render workloads A, B, Bp, C of --impl ours")
     if args.impl == "reference":
         if args.workload in ("D", "E", "sweep", "train", "decoder"):
             args.workload = "B"
@@ -1107,13 +1132,13 @@ def run_decoder(args, rank, world, local_rank):
     pix_sphere = torch.stack([torch.round(pix[:, 0] * ((oW - 1) / (W - 1))), torch.round(pix[:, 1] * ((oH - 1) / (H - 1)))], 1).long()
     ms = time_loop(lambda: dec(features, pix, pix_sphere), args.steps, args.warmup, torch.cuda.synchronize)
     peaks = load_peaks()
-    peak = float(peaks.get("bf16_tflops_sustained") or 1400.0) / 2.0
+    peak = float(peaks.get("bf16_tflops_sustained") or H100_FP16_TFLOPS) / 2.0
     if rank == 0:
         print(json.dumps({"metric": "decoder images/sec (DecoderSphere.forward of one 1220x370 KITTI image -> packed 1500x452 pyramid)",
                           "value": 1e3 / ms, "unit": "images/s", "ms_per_step": ms, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
                           "dtype": "tf32 operands (rounded to nearest), fp32 storage and accumulate", "data": "synthetic", "higher_is_better": True,
                           "gpu_launches": int(dec.launches) + 18,
-                          "roofline": {"bound": "tensor (tcgen05 kind::tf32; peak = measured bf16 sustained / 2)", "achieved": flop / (ms * 1e-3) / 1e12,
+                          "roofline": {"bound": "tensor (wgmma tf32; peak = fp16 peak / 2)", "achieved": flop / (ms * 1e-3) / 1e12,
                                        "peak": peak, "unit": "TFLOP/s", "frac": flop / (ms * 1e-3) / 1e12 / peak,
                                        "algorithmic_flop_per_step": flop,
                                        "note": "whole step incl. conv2 (PyTorch), the sphere resamplings and the upsample+concat kernels; "

@@ -1,5 +1,5 @@
 /*
- * scenerf_b200 -- C ABI of the Blackwell (sm_100a) ray renderer that replaces the hot path of
+ * scenerf_b200 -- C ABI of the Hopper (sm_90a) ray renderer that replaces the hot path of
  * astra-vision/SceneRF: `SceneRF.render_rays_batch` (reference scenerf/models/scenerf.py:392-471, BundleFusion twin
  * scenerf/models/scenerf_bf.py:420-494) and everything below it.
  *
@@ -41,9 +41,9 @@ enum srf_status {
 
 enum srf_precision {
   SRF_PREC_FP32 = 0, /* SIMT fp32 FMA everywhere: strict mode, matches the reference to float32 round-off */
-  SRF_PREC_FP16_TC = 1, /* tcgen05 tensor cores: fp16 operands, fp32 accumulate in TMEM ("fast mode") */
-  SRF_PREC_FP32_TC = 2  /* tcgen05 tensor cores at float32-grade accuracy: every fp32 operand is carried as an fp16
-                           hi/lo pair (22 mantissa bits), all four partial products accumulate in fp32 in TMEM.
+  SRF_PREC_FP16_TC = 1, /* wgmma tensor cores: fp16 operands, fp32 accumulate ("fast mode") */
+  SRF_PREC_FP32_TC = 2  /* wgmma tensor cores at float32-grade accuracy: every fp32 operand is carried as an fp16
+                           hi/lo pair (22 mantissa bits), all four partial products accumulate in fp32.
                            The precision-matched mode for the reference's fp32 sgemm (resnetfc.py:54-63,133-164);
                            needs an SRF_PYR_FP32 pyramid and srf_pack_weights_tc_split() output */
 };
@@ -108,11 +108,11 @@ typedef struct srf_config {
 } srf_config;
 
 #define SRF_FLAG_HIDDEN_FP16 2       /* tensor-core path: the residual hidden state h travels between ResNet blocks as
-                                       fp16 instead of fp32 (GEMM accumulation stays fp32 in TMEM).  Halves the
+                                       fp16 instead of fp32 (GEMM accumulation stays fp32).  Halves the
                                        L2 traffic of the epilogues; h is rounded to fp16 as the next GEMM's operand
                                        anyway, measured effect on depth/colour error < 15 % of the fp16-mode error */
 #define SRF_FLAG_TF32_MATMUL 8      /* float32 path, training (needs SRF_FLAG_SAVE_ACTIVATIONS in the forward): the GEMMs of the
-                                       forward and of srf_render_rays_backward run on tensor cores as tcgen05 kind::tf32
+                                       forward and of srf_render_rays_backward run on tensor cores as wgmma tf32
                                        (float32 storage, 10-bit mantissa operands, float32 accumulate) -- the regime of the
                                        reference's own torch 1.7.1 defaults on Ampere-class GPUs.  Not bit-compatible with
                                        the strict float32 mode; tolerances in DESIGN.md 6.3. */
@@ -276,7 +276,7 @@ int srf_sphere_feature(const float* x_chw_dev, int C, int h, int w, const float*
  *   srf_conv3x3_hwc         : y = LeakyReLU_slope( conv3x3(in; dilation = padding = dil) * scale + shift (+ residual) ); slope 1 = none.
  *                             w9_dev: weights repacked [9][Cout][ld_in] (tap = ky*3 + kx; Conv2d.weight[co][ci][ky][kx]), zero for
  *                             padded ci.  Writes out32_dev (H,W,ld32) float32 and/or out16_dev (H,W,ld16) IEEE half -- with
- *                             ld = Cout these ARE the buffers srf_pyramid.hwc[] points to (no CHW->HWC pass).  tcgen05 kind::tf32
+ *                             ld = Cout these ARE the buffers srf_pyramid.hwc[] points to (no CHW->HWC pass).  wgmma tf32
  *                             implicit GEMM, operands read as fp32 with a 10-bit mantissa (cuDNN's default allow_tf32 regime).  The
  *                             tensor core truncates; feed it tensors already rounded to the nearest tf32 value (w9 rounded by the
  *                             caller; round_out != 0 stores out32 rounded because it feeds another convolution; the concat kernel
@@ -288,7 +288,7 @@ int srf_conv3x3_hwc(const float* in_dev, int H, int W, int ld_in, const float* w
                     void* out16_dev, int ld16, void* stream);
 
 /* Diagnostic: one GEMM of the training path, C[M x N] = epilogue(A[M x K] * B[N x K]^T) with float32 device operands.
- * use_tf32 != 0 runs the tcgen05 kind::tf32 kernel (csrc/gemm_tf32.cu), 0 the float32 SIMT kernel (csrc/gemm.cu).
+ * use_tf32 != 0 runs the wgmma tf32 kernel (csrc/gemm_tf32.cu), 0 the float32 SIMT kernel (csrc/gemm.cu).
  * bias (N) / mask (M x N, keeps values where mask > 0) / residual (M x N) may be NULL; splitk_ws enables split-K. */
 int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K, const float* bias,
                    const float* mask, int ldm, const float* residual, int ldr, int accumulate, float* splitk_ws,

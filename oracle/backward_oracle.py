@@ -48,7 +48,7 @@ def taps_2d(coords, norm_size, H, W):
 
 
 def tf32_trunc(a):
-    """Operand rounding of tcgen05 kind::tf32: the float32 value with its low 13 mantissa bits dropped."""
+    """Operand rounding of the tf32 tensor-core MMA (wgmma .tf32): the float32 value with its low 13 mantissa bits dropped."""
     u = np.ascontiguousarray(a, dtype=f32).view(np.uint32) & np.uint32(0xFFFFE000)
     return u.view(f32).astype(f64)
 

@@ -143,7 +143,7 @@ class TrainableRenderer:
     def __init__(self, hp: dict, mlp, mlp_gaussian, device="cuda:0", rng: str = "torch", save_activations: bool = True,
                  matmul: str = "fp32"):
         if matmul not in ("fp32", "tf32"):
-            raise ValueError("matmul must be 'fp32' (strict SIMT) or 'tf32' (tcgen05 tensor cores)")
+            raise ValueError("matmul must be 'fp32' (strict SIMT) or 'tf32' (wgmma tensor cores)")
         state = lambda m: dict(m.named_parameters()) if hasattr(m, "named_parameters") else dict(m)
         self.mlp, self.mlp_gaussian = mlp, mlp_gaussian
         self._state = state
@@ -153,7 +153,7 @@ class TrainableRenderer:
         # True: keep the ResnetFC pre-activations of the forward (24.4 KB per sample point) for the backward;
         # False: recompute them chunk by chunk in the backward (less memory, ~25 % more arithmetic)
         self.renderer.save_activations = bool(save_activations)
-        # "tf32": the GEMMs of the training forward and of the backward run as tcgen05 kind::tf32 (float32 storage, 10-bit
+        # "tf32": the GEMMs of the training forward and of the backward run as wgmma tf32 (float32 storage, 10-bit
         # mantissa operands) -- several times faster, not bit-compatible with the strict mode (DESIGN.md 6.3)
         self.renderer.tf32_matmul = matmul == "tf32"
 
@@ -183,7 +183,7 @@ class TrainableRenderer:
 
 
 def patch_for_training(model, rng: str = "torch", matmul: str = "fp32"):
-    """Route `model.render_rays_batch` of a reference SceneRF module through the differentiable B200 path: gradients
+    """Route `model.render_rays_batch` of a reference SceneRF module through the differentiable CUDA path: gradients
     reach model.mlp, model.mlp_gaussian and (through x_rgb) the image encoder.  Returns the TrainableRenderer."""
     base = B200Renderer.from_module(model, precision="fp32", rng=rng)
     t = TrainableRenderer(base.hp, model.mlp, model.mlp_gaussian, device=base.device, rng=rng, matmul=matmul)

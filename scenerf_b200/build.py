@@ -1,4 +1,4 @@
-"""Builds libscenerf_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libscenerf_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m scenerf_b200.build [--force]
 
@@ -15,7 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libscenerf_b200.so")
 SOURCES = ["api.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_tc.cu", "pack.cu", "tsdf.cu", "image_ops.cu", "backward.cu", "gemm.cu", "sphere_feature.cu", "gemm_tf32.cu", "preproj.cu", "conv_tf32.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*GENCODE, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -73,7 +74,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         log.append("== %s ==\n%s" % (src, out))
         if pr.returncode:
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out))
-    cmd = [_nvcc(), "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", LIB_PATH, *objs, *GENCODE]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode:
         raise RuntimeError("link failed:\n" + r.stdout)
@@ -97,7 +98,7 @@ def build_variant(name: str, defines) -> str:
         raise RuntimeError("nvcc failed:\n" + r.stdout)
     objs = [obj if s == "mlp_tc.cu" else os.path.join(HERE, "build", s.replace(".cu", ".o")) for s in SOURCES]
     out = os.path.join(HERE, "libscenerf_b200_%s.so" % name)
-    r = subprocess.run([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a"], stdout=subprocess.PIPE,
+    r = subprocess.run([_nvcc(), "-shared", "-o", out, *objs, *GENCODE], stdout=subprocess.PIPE,
                        stderr=subprocess.STDOUT, text=True)
     if r.returncode:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -213,7 +213,7 @@ struct GemmOpt {
   const int* seg_flags = nullptr; int seg_mode = 0; const int* seg_off = nullptr;     // tf32 kernel: fused per-scale segments
   float* relu_out = nullptr; int ld_relu = 0;                                         // tf32 kernel: also store max(result, 0)
 };
-// SRF_FLAG_TF32_MATMUL: NT GEMMs without operand ReLU go to the tcgen05 kind::tf32 kernel (gemm_tf32.cu); the callers
+// SRF_FLAG_TF32_MATMUL: NT GEMMs without operand ReLU go to the wgmma tf32 kernel (gemm_tf32.cu); the callers
 // below arrange their operands accordingly (ReLU'd / transposed copies).  Set per call by the run_* entry points.
 static thread_local bool g_tf32 = false;
 

@@ -1,4 +1,4 @@
-// Shared device-side definitions for the SceneRF ray-render kernels (sm_100a).
+// Shared device-side definitions for the SceneRF ray-render kernels (sm_90a).
 //
 // The per-point geometry below restates, operation by operation, what the reference does in
 //   utils.py:298-315 (cam_pts_2_pix), spherical_mapping.py:8-18,80-115 (pixel -> integer sphere coords),

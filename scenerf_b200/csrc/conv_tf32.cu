@@ -9,26 +9,28 @@
 //   TMA's out-of-bounds zero fill IS the convolution's zero padding (negative / too large coordinates), and the box lands
 //   in shared memory as the same 128-row x 128-byte swizzled tile a plain GEMM would stage.
 //   B tiles: 2-D map over the weights repacked [tap][co][ci] (ci padded to a multiple of 4), box {32, 128} at (c0, tap*Cout + n0).
-//   tcgen05.mma kind::tf32 (fp32 operands read in place, 10-bit mantissa -- the regime of the reference's own cuDNN default
-//   `allow_tf32=True` on Ampere-class GPUs), fp32 accumulator in TMEM, 3-stage mbarrier ring, one elected issuer thread.
+//   wgmma .tf32 (fp32 operands read in place, 10-bit mantissa -- the regime of the reference's own cuDNN default
+//   `allow_tf32=True` on Ampere-class GPUs), 3-stage mbarrier ring fed by one TMA thread, two consumer warpgroups that each
+//   accumulate 64 pixels x 128 channels in registers (wgmma m64n128k8).
 //   The tensor core TRUNCATES the 13 low mantissa bits of what it reads; through the decoder's 35 chained convolutions that
 //   bias compounds (1.3 % relative L2 on the finest map of the test network).  So every tensor that feeds a convolution is
 //   stored already ROUNDED TO NEAREST tf32 (weights at pack time, the concat buffer, intermediate activations: `round_out`),
 //   which makes the truncation exact: 0.2 % relative L2, 6.7x better, at no cost.  The pyramid maps themselves stay unrounded.
-//   Epilogue (4 warps, tcgen05.ld): y = acc*scale[co] + shift[co] (conv bias + eval-mode BatchNorm folded on the host),
+//   Epilogue (from the accumulator registers): y = acc*scale[co] + shift[co] (conv bias + eval-mode BatchNorm folded on the host),
 //   (+ residual[p, co]), LeakyReLU, store fp32 [H][W][C] and/or fp16 [H][W][C] -- i.e. straight into the packed pyramid
 //   layout of srf_pyramid (no CHW -> HWC pass).
-// Roofline: tensor (tf32 = half the kind::f16 rate); 2*9*Cin*Cout flops per pixel.
+// Roofline: tensor (tf32 = half the f16 rate); 2*9*Cin*Cout flops per pixel.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace srf {
 namespace conv {
 
 constexpr int kBM = 128, kBN = 128, kBK = 32, kStages = 3;
 constexpr uint32_t kTileBytes = kBM * kBK * 4;            // 16 KB
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;                             // warpgroup 0: TMA producer (one thread); 1, 2: MMA + epilogue
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -58,37 +60,9 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (same encoding as mlp_tc.cu: make_desc_sw128)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// instruction descriptor: c_format F32 (1) at [4,6), a/b format TF32 (2) at [7,10) / [10,13), K-major, N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kBN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
 
 struct ConvArgs {
   int H, W, Cin, Cout;            // Cin as stored (channel stride of the input, multiple of 4; padded channels hold zeros)
@@ -107,14 +81,13 @@ struct ConvArgs {
 // nearest value with a 10-bit mantissa (ties away from zero; finite inputs)
 __device__ __forceinline__ float round_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
 
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 1)
 conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvArgs a) {
   extern __shared__ unsigned char smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;            // SWIZZLE_128B tiles need 1024-byte alignment
   const uint32_t sA = base, sB = base + kStages * kTileBytes;
-  const uint32_t bars = sB + kStages * kTileBytes;                        // full[kStages], empty[kStages], acc
-  const uint32_t tmem_slot = bars + 8u * (2 * kStages + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t bars = sB + kStages * kTileBytes;                        // full[kStages], empty[kStages]
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int xt = (a.W + kBM - 1) / kBM;
   const int y = blockIdx.y / xt, x0 = (blockIdx.y % xt) * kBM;
   const int n0 = blockIdx.x * kBN;
@@ -124,22 +97,13 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    for (int s = 0; s < kStages; ++s) { mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (kStages + s), 1); }
-    mbar_init(bars + 8u * (2 * kStages), 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (kStages + s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(128u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (t == 0) {
       for (int j = 0; j < nk; ++j) {
         const int tap = j / kb, cb = j - tap * kb;
         const int dy = (tap / 3 - 1) * a.dil, dx = (tap % 3 - 1) * a.dil;
@@ -150,64 +114,51 @@ conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         tma_load_2d(sB + s * kTileBytes, &tmB, cb * kBK, tap * a.Cout + n0, bars + 8u * s);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int j = 0; j < nk; ++j) {
-        const int s = j % kStages;
-        mbar_wait(bars + 8u * s, ((uint32_t)(j / kStages)) & 1u, a.err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k4 = 0; k4 < kBK / 8; ++k4)
-          umma_tf32(tmem, make_desc_sw128(sA + s * kTileBytes + k4 * 32), make_desc_sw128(sB + s * kTileBytes + k4 * 32), kIdesc,
-                    (j > 0 || k4 > 0) ? 1u : 0u);
-        umma_commit(bars + 8u * (kStages + s));
-      }
-      umma_commit(bars + 8u * (2 * kStages));
-    }
-  } else {
-    const int q = warp & 3;                                 // TMEM lane quarter this warp may read
-    const int px = x0 + q * 32 + lane;
-    const size_t pix = (size_t)y * a.W + px;
-    mbar_wait(bars + 8u * (2 * kStages), 0, a.err);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c = 0; c < kBN / 32; ++c) {
-      if (n0 + c * 32 >= a.Cout) break;                     // warp-uniform
-      uint32_t v[32];
-      tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (px < a.W) {
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const int co = n0 + c * 32 + j4 * 4;
-          if (co >= a.Cout) break;                          // Cout % 4 == 0
-          const float4 sc = __ldg(reinterpret_cast<const float4*>(a.scale + co)), sh = __ldg(reinterpret_cast<const float4*>(a.shift + co));
-          float4 o = make_float4(fmaf(__uint_as_float(v[j4 * 4]), sc.x, sh.x), fmaf(__uint_as_float(v[j4 * 4 + 1]), sc.y, sh.y),
-                                 fmaf(__uint_as_float(v[j4 * 4 + 2]), sc.z, sh.z), fmaf(__uint_as_float(v[j4 * 4 + 3]), sc.w, sh.w));
-          if (a.residual) {
-            const float4 t = *reinterpret_cast<const float4*>(a.residual + pix * a.ld_res + co);
-            o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w;
-          }
-          o.x = o.x > 0.f ? o.x : o.x * a.slope; o.y = o.y > 0.f ? o.y : o.y * a.slope;
-          o.z = o.z > 0.f ? o.z : o.z * a.slope; o.w = o.w > 0.f ? o.w : o.w * a.slope;
-          if (a.out16) {
-            __half2* d = reinterpret_cast<__half2*>(a.out16 + pix * a.ld16 + co);
-            d[0] = __floats2half2_rn(o.x, o.y);
-            d[1] = __floats2half2_rn(o.z, o.w);
-          }
-          if (a.out32) {
-            if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-            *reinterpret_cast<float4*>(a.out32 + pix * a.ld32 + co) = o;
-          }
-        }
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u) : "memory");
+  // consumer warpgroup: pixels x0 + (wg - 1) * 64 .. +63 (the A tile's 64-row half starts 8 KB further)
+  const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int j = 0; j < nk; ++j) {
+    const int s = j % kStages;
+    mbar_wait(bars + 8u * s, ((uint32_t)(j / kStages)) & 1u, a.err);
+    gmma::fence();
+#pragma unroll
+    for (int k4 = 0; k4 < kBK / 8; ++k4)
+      gmma::mma_tf32_n128(acc, gmma::desc_sw128(sA + s * kTileBytes + a_off + k4 * 32), gmma::desc_sw128(sB + s * kTileBytes + k4 * 32),
+                          (j > 0 || k4 > 0) ? 1 : 0);
+    gmma::commit();
+    // this stage's MMAs stay in flight; the previous stage has completed and goes back to the producer
+    gmma::wait<1>();
+    if (t == 0 && j > 0) mbar_arrive(bars + 8u * (kStages + (j - 1) % kStages));
+  }
+  gmma::wait<0>();
+  gmma::fence_regs(acc);
+  const int w = t >> 5, l = t & 31;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int px = x0 + (wg - 1) * 64 + 16 * w + (l >> 2) + 8 * half;
+    if (px >= a.W) continue;
+    const size_t pix = (size_t)y * a.W + px;
+#pragma unroll
+    for (int c8 = 0; c8 < kBN / 8; ++c8) {
+      const int co = n0 + 8 * c8 + 2 * (l & 3);
+      if (co >= a.Cout) break;                              // Cout % 4 == 0: co + 1 < Cout as well
+      const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + co)), sh = __ldg(reinterpret_cast<const float2*>(a.shift + co));
+      float2 o = make_float2(fmaf(acc[4 * c8 + 2 * half], sc.x, sh.x), fmaf(acc[4 * c8 + 2 * half + 1], sc.y, sh.y));
+      if (a.residual) {
+        const float2 t2 = *reinterpret_cast<const float2*>(a.residual + pix * a.ld_res + co);
+        o.x += t2.x; o.y += t2.y;
+      }
+      o.x = o.x > 0.f ? o.x : o.x * a.slope; o.y = o.y > 0.f ? o.y : o.y * a.slope;
+      if (a.out16) *reinterpret_cast<__half2*>(a.out16 + pix * a.ld16 + co) = __floats2half2_rn(o.x, o.y);
+      if (a.out32) {
+        if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); }
+        *reinterpret_cast<float2*>(a.out32 + pix * a.ld32 + co) = o;
+      }
+    }
   }
 }
 
@@ -296,7 +247,7 @@ int launch_conv3x3_tf32(const float* in, int H, int W, int Cin, const float* w9,
     if (cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped) == cudaSuccess) { *h = 0; cudaHostGetDevicePointer(&g_conv_err, h, 0); }
   }
   static bool attr = false;
-  const size_t smem = 2 * conv::kStages * conv::kTileBytes + 1024 + 256;
+  const size_t smem = 2 * conv::kStages * conv::kTileBytes + 1024 + 64;
   if (!attr) { cudaFuncSetAttribute(conv::conv3x3_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
   conv::ConvArgs a;
   a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.dil = dil; a.scale = scale; a.shift = shift; a.residual = residual; a.ld_res = ld_res;

@@ -6,7 +6,7 @@
 //   epilogue: v = acc (+bias[n]); if mask: v = mask[m][n] > 0 ? v : 0; if R: v += R[m][n]; if accumulate: v += C[m][n]
 // gemm128_kernel: 128x128x16 tiles, 8x8 outputs per thread, float4 global/shared accesses, register-prefetched double
 // buffering -- the hot one (needs 16-byte aligned rows).  gemm64_kernel: 64x64x16, scalar loads, any shape (lin_in K=42,
-// lin_out M=4 ...).  FP32-FMA-bound: 2*M*N*K flops against 148 SMs x 128 lanes x 2 x clock.
+// lin_out M=4 ...).  FP32-FMA-bound: 2*M*N*K flops against SMs (132 on an H100 SXM) x 128 lanes x 2 x clock.
 #include "kernels.cuh"
 
 namespace srf {
@@ -203,6 +203,19 @@ splitk_reduce_kernel(const float* __restrict__ part, int splits, float* __restri
   *dst = accumulate ? (*dst + v) : v;
 }
 
+int device_sm_count() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      n = 132;                 // no device visible (size queries on a build machine): H100 SXM
+      cudaGetLastError();
+    }
+  }
+  return n;
+}
+
 int& launch_counter() {
   static thread_local int c = 0;
   return c;
@@ -226,7 +239,7 @@ static void dispatch(const GemmArgs& g, cudaStream_t st) {
     const int tiles = grid.x * grid.y;
     int splits = 1;
     if (g.splitk_ws && !g.bias && !g.mask && !g.R && tiles < 96 && g.K >= 1024) {
-      splits = (2 * 148 + tiles - 1) / tiles;
+      splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
       if (splits > 16) splits = 16;
       while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
     }
@@ -248,7 +261,7 @@ static void dispatch(const GemmArgs& g, cudaStream_t st) {
     const int tiles = grid.x * grid.y;
     int splits = 1;
     if (g.splitk_ws && !g.bias && !g.mask && !g.R && tiles < 96 && g.K >= 1024) {
-      splits = (2 * 148 + tiles - 1) / tiles;
+      splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
       if (splits > 64) splits = 64;
       while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
     }

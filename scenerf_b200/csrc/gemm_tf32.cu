@@ -1,21 +1,20 @@
 // TF32 tensor-core GEMM for the training path:  C[M x N] = epilogue( A[M x K] * B[N x K]^T ),  A and B float32, both
-// K-contiguous ("NT"), accumulation in float32 in tensor memory.  tcgen05.mma kind::tf32 reads the float32 operands
-// straight from shared memory (top 19 bits), so there is no conversion pass: TMA (cp.async.bulk.tensor.2d, 128-byte
-// swizzle) stages 128 x 32 float tiles of A and B, one elected thread issues 4 MMAs (K = 8 each) per stage into a
-// 128 x 128 fp32 accumulator (128 TMEM columns), tcgen05.commit releases the stage, 4 epilogue warps read the
-// accumulator with tcgen05.ld and apply the same epilogue as gemm.cu (bias, ReLU mask, residual, accumulate).
-// One output tile per CTA, 3 stages (96 KB) so that two CTAs share an SM and one's epilogue overlaps the other's main
-// loop; split-K over gridDim.z with fixed-order reduction for the weight-gradient shapes.
-// Roofline: tensor pipe (tf32 = half the f16 rate) -- and L2->SM bandwidth: a 128x128 tile moves 32 KB per 1.05 MFLOP.
+// K-contiguous ("NT"), accumulation in float32.  wgmma .tf32 reads the float32 operands straight from shared memory (top 19
+// bits), so there is no conversion pass: TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) stages 128 x 32 float tiles of A
+// and B into a 3-stage mbarrier ring, and two consumer warpgroups (rows 0-63 / 64-127 of the tile) each issue 4 wgmma
+// m64n128k8 per stage into a 64 x 128 register accumulator, then apply the same epilogue as gemm.cu (bias, ReLU mask,
+// residual, accumulate) straight from registers.  One output tile per CTA; split-K over gridDim.z with fixed-order
+// reduction for the weight-gradient shapes.
 #include <cuda.h>
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace srf {
 namespace tf32 {
 
 constexpr int kBM = 128, kBN = 128, kBK = 32, kStages = 3;
 constexpr uint32_t kTileBytes = kBM * kBK * 4;            // 16 KB
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;                             // warpgroup 0: TMA producer (one thread); 1, 2: MMA + epilogue
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -23,6 +22,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -42,37 +44,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (same encoding as mlp_tc.cu: make_desc_sw128)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// instruction descriptor: c_format F32 (1) at [4,6), a/b format TF32 (2) at [7,10) / [10,13), K-major, N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kBN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
 
 struct SegInfo { const int* flags; int mode; int off[6]; };
 // true when [lo, hi) of the latent axis touches only scales whose flag is 0
@@ -83,7 +54,7 @@ __device__ __forceinline__ bool seg_dead(const SegInfo& sg, int lo, int hi) {
   return true;
 }
 
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* C, int ldc, int M, int N,
                     int K, const float* __restrict__ bias, const float* __restrict__ mask, int ldm, const float* R, int ldr,
                     int accumulate, int k_per, const int* __restrict__ skip, const __grid_constant__ SegInfo sg, int* err,
@@ -93,9 +64,8 @@ gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   extern __shared__ unsigned char smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;            // SWIZZLE_128B tiles need 1024-byte alignment
   const uint32_t sA = base, sB = base + kStages * kTileBytes;
-  const uint32_t bars = sB + kStages * kTileBytes;                        // full[kStages], empty[kStages], acc
-  const uint32_t tmem_slot = bars + 8u * (2 * kStages + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t bars = sB + kStages * kTileBytes;                        // full[kStages], empty[kStages]
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * kBN;
   const int kbeg = blockIdx.z * k_per;
   const int kend = min(K, kbeg + k_per);
@@ -105,29 +75,20 @@ gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");   // descriptor fetch off the first load's path
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    for (int s = 0; s < kStages; ++s) { mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (kStages + s), 1); }
-    mbar_init(bars + 8u * (2 * kStages), 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (kStages + s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(128u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
 
-  // K-segmented mode: k-blocks that lie entirely in dead scales are skipped by producer and issuer alike (same predicate,
+  // K-segmented mode: k-blocks that lie entirely in dead scales are skipped by producer and consumers alike (same predicate,
   // same order, so the ring stays in step); n_live = number of blocks actually streamed
   int n_live = nk;
   if (sg.mode == 1) {
     n_live = 0;
     for (int i = 0; i < nk; ++i) n_live += seg_dead(sg, kbeg + i * kBK, min(kend, kbeg + (i + 1) * kBK)) ? 0 : 1;
   }
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (t == 0) {
       int j = 0;
       for (int i = 0; i < nk; ++i) {
         if (sg.mode == 1 && seg_dead(sg, kbeg + i * kBK, min(kend, kbeg + (i + 1) * kBK))) continue;
@@ -139,238 +100,50 @@ gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         ++j;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int j = 0; j < n_live; ++j) {
-        const int s = j % kStages;
-        mbar_wait(bars + 8u * s, ((uint32_t)(j / kStages)) & 1u, err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k4 = 0; k4 < kBK / 8; ++k4)
-          umma_tf32(tmem, make_desc_sw128(sA + s * kTileBytes + k4 * 32), make_desc_sw128(sB + s * kTileBytes + k4 * 32), kIdesc,
-                    (j > 0 || k4 > 0) ? 1u : 0u);
-        umma_commit(bars + 8u * (kStages + s));            // stage free once these MMAs have read it
-      }
-      if (n_live > 0) umma_commit(bars + 8u * (2 * kStages));   // accumulator complete
-    }
-  } else {
-    const int q = warp & 3;                                 // TMEM lane quarter this warp may read
-    const int gm = m0 + q * 32 + lane;
-    if (n_live > 0) mbar_wait(bars + 8u * (2 * kStages), 0, err);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c = 0; c < kBN / 32; ++c) {
-      uint32_t v[32];
-      if (n_live > 0) {
-        tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0u;
-      }
-      if (gm < M) {
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const int gn = n0 + c * 32 + j4 * 4;
-          if (gn >= N) break;                              // N % 4 == 0
-          float4 o = make_float4(__uint_as_float(v[j4 * 4]), __uint_as_float(v[j4 * 4 + 1]), __uint_as_float(v[j4 * 4 + 2]),
-                                 __uint_as_float(v[j4 * 4 + 3]));
-          if (bias) { const float4 t = *reinterpret_cast<const float4*>(bias + gn); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-          if (mask) {
-            const float4 t = *reinterpret_cast<const float4*>(mask + (size_t)gm * ldm + gn);
-            o.x = t.x > 0.f ? o.x : 0.f; o.y = t.y > 0.f ? o.y : 0.f; o.z = t.z > 0.f ? o.z : 0.f; o.w = t.w > 0.f ? o.w : 0.f;
-          }
-          if (R) { const float4 t = *reinterpret_cast<const float4*>(R + (size_t)gm * ldr + gn); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-          float4* dst = reinterpret_cast<float4*>(C + (size_t)gm * ldc + gn);
-          if (accumulate) { const float4 t = *dst; o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-          *dst = o;
-          if (relu_out)          // the consumer GEMM reads its A operand as stored: hand it the ReLU'd activations directly
-            *reinterpret_cast<float4*>(relu_out + (size_t)gm * ld_relu + gn) = make_float4(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f), fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
-        }
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------------------------
-// v2: persistent, 128 x 256 output tiles, 4-stage ring (A 16 KB + B 32 KB per stage), two 256-column accumulators in TMEM so that
-// the epilogue of tile i runs under the main loop of tile i+1.  Why: kind::tf32 reads fp32 operands (4 B / element) from shared
-// memory, so the GEMM is bound by L2 -> SM bytes, not by the tensor pipe: a 128 x 128 x 32 step moves 32 KB per 1.05 MFLOP
-// (32 flop/B -> at ~42 B/cycle/SM of L2 bandwidth 33 % of the tf32 rate at best); 128 x 256 moves 48 KB per 2.1 MFLOP (43.7 flop/B)
-// and one CTA per SM keeps 192 KB in flight.  Same contract as gemm_tf32_nt_kernel (bias / ReLU mask / residual / accumulate /
-// ReLU'd side output, dead-scale segments, deterministic split-K); tiles are taken round-robin, n fastest (neighbouring CTAs
-// share the A rows in L2).
-constexpr int k2BN = 256, k2Stages = 4;
-constexpr uint32_t k2ABytes = kBM * kBK * 4, k2BBytes = k2BN * kBK * 4, k2StageBytes = k2ABytes + k2BBytes;      // 16 + 32 KB
-constexpr uint32_t k2Idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(k2BN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tf32_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* C, int ldc, int M, int N,
-                            int K, const float* __restrict__ bias, const float* __restrict__ mask, int ldm, const float* R, int ldr,
-                            int accumulate, int k_per, int splits, const int* __restrict__ skip, const __grid_constant__ SegInfo sg, int* err,
-                            float* relu_out, int ld_relu) {
-  if (skip && *skip == 0) return;
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = base + k2Stages * k2StageBytes;            // full[4], empty[4], acc_full[2], acc_empty[2]
-  auto full = [&](int s_) { return bars + 8u * s_; };
-  auto empty = [&](int s_) { return bars + 8u * (k2Stages + s_); };
-  auto acc_full = [&](int b_) { return bars + 8u * (2 * k2Stages + b_); };
-  auto acc_empty = [&](int b_) { return bars + 8u * (2 * k2Stages + 2 + b_); };
-  const uint32_t tmem_slot = bars + 8u * (2 * k2Stages + 4);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mt = (M + kBM - 1) / kBM, nt = (N + k2BN - 1) / k2BN;
-  const int total = mt * nt * splits;
-
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    for (int s_ = 0; s_ < k2Stages; ++s_) { mbar_init(full(s_), 1); mbar_init(empty(s_), 1); }
-    for (int b_ = 0; b_ < 2; ++b_) { mbar_init(acc_full(b_), 1); mbar_init(acc_empty(b_), 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
-
-  // tile t -> (split z, row tile m, column tile n); every role walks the same sequence and applies the same skips
-  struct Tile { int m0, n0, kbeg, kend, z; bool dead; };
-  auto tile_of = [&](int t) {
-    Tile tl;
-    const int n = t % nt, m = (t / nt) % mt;
-    tl.z = t / (nt * mt);
-    tl.m0 = m * kBM; tl.n0 = n * k2BN;
-    tl.kbeg = tl.z * k_per; tl.kend = min(K, tl.kbeg + k_per);
-    tl.dead = (sg.mode == 2) && seg_dead(sg, tl.n0, min(N, tl.n0 + k2BN));
-    return tl;
-  };
-  auto block_dead = [&](const Tile& tl, int i) {
-    return sg.mode == 1 && seg_dead(sg, tl.kbeg + i * kBK, min(tl.kend, tl.kbeg + (i + 1) * kBK));
-  };
-  auto live_blocks = [&](const Tile& tl) {
-    const int nk = (tl.kend - tl.kbeg + kBK - 1) / kBK;
-    if (sg.mode != 1) return nk;
-    int c = 0;
-    for (int i = 0; i < nk; ++i) c += block_dead(tl, i) ? 0 : 1;
-    return c;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int j = 0;                                             // stages issued so far (ring position)
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const Tile tl = tile_of(t);
-        if (tl.dead) continue;
-        const int nk = (tl.kend - tl.kbeg + kBK - 1) / kBK;
-        for (int i = 0; i < nk; ++i) {
-          if (block_dead(tl, i)) continue;
-          const int s_ = j % k2Stages;
-          mbar_wait(empty(s_), (((uint32_t)(j / k2Stages)) & 1u) ^ 1u, err);
-          mbar_arrive_expect_tx(full(s_), k2StageBytes);
-          tma_load_2d(base + s_ * k2StageBytes, &tmA, tl.kbeg + i * kBK, tl.m0, full(s_));
-          tma_load_2d(base + s_ * k2StageBytes + k2ABytes, &tmB, tl.kbeg + i * kBK, tl.n0, full(s_));
-          ++j;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int j = 0, at = 0;                                     // ring position, accumulator-tile counter
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const Tile tl = tile_of(t);
-        if (tl.dead) continue;
-        const int n_live = live_blocks(tl);
-        if (n_live == 0) continue;                           // the epilogue writes zeros without an accumulator
-        const int buf = at & 1;
-        mbar_wait(acc_empty(buf), (((uint32_t)(at >> 1)) & 1u) ^ 1u, err);       // the epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int i = 0; i < n_live; ++i) {
-          const int s_ = j % k2Stages;
-          mbar_wait(full(s_), ((uint32_t)(j / k2Stages)) & 1u, err);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t sa = base + s_ * k2StageBytes, sb = sa + k2ABytes;
+  // consumer warpgroup: rows (wg - 1) * 64 .. +63 of the tile (the A tile's 64-row half starts 8 KB further)
+  const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;
+  float acc[64];
 #pragma unroll
-          for (int k4 = 0; k4 < kBK / 8; ++k4)
-            umma_tf32(tmem + (uint32_t)(buf * k2BN), make_desc_sw128(sa + k4 * 32), make_desc_sw128(sb + k4 * 32), k2Idesc,
-                      (i > 0 || k4 > 0) ? 1u : 0u);
-          umma_commit(empty(s_));
-          ++j;
-        }
-        umma_commit(acc_full(buf));
-        ++at;
-      }
-    }
-  } else {
-    const int q = warp & 3;                                  // TMEM lane quarter this warp may read
-    int at = 0;
-    for (int t = blockIdx.x; t < total; t += gridDim.x) {
-      const Tile tl = tile_of(t);
-      if (tl.dead) continue;
-      const int n_live = live_blocks(tl);
-      const int buf = at & 1;
-      if (n_live > 0) {
-        mbar_wait(acc_full(buf), ((uint32_t)(at >> 1)) & 1u, err);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      const int gm = tl.m0 + q * 32 + lane;
-      float* Cz = (splits > 1) ? C + (size_t)tl.z * M * ldc : C;
-#pragma unroll 1
-      for (int c = 0; c < k2BN / 32; ++c) {
-        if (tl.n0 + c * 32 >= N) break;                      // warp-uniform
-        uint32_t v[32];
-        if (n_live > 0) {
-          tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * k2BN + c * 32), v);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int j = 0; j < n_live; ++j) {
+    const int s = j % kStages;
+    mbar_wait(bars + 8u * s, ((uint32_t)(j / kStages)) & 1u, err);
+    gmma::fence();
 #pragma unroll
-          for (int j2 = 0; j2 < 32; ++j2) v[j2] = 0u;
-        }
-        if (gm < M) {
-#pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) {
-            const int gn = tl.n0 + c * 32 + j4 * 4;
-            if (gn >= N) break;                              // N % 4 == 0
-            float4 o = make_float4(__uint_as_float(v[j4 * 4]), __uint_as_float(v[j4 * 4 + 1]), __uint_as_float(v[j4 * 4 + 2]),
-                                   __uint_as_float(v[j4 * 4 + 3]));
-            if (bias) { const float4 t4 = *reinterpret_cast<const float4*>(bias + gn); o.x += t4.x; o.y += t4.y; o.z += t4.z; o.w += t4.w; }
-            if (mask) {
-              const float4 t4 = *reinterpret_cast<const float4*>(mask + (size_t)gm * ldm + gn);
-              o.x = t4.x > 0.f ? o.x : 0.f; o.y = t4.y > 0.f ? o.y : 0.f; o.z = t4.z > 0.f ? o.z : 0.f; o.w = t4.w > 0.f ? o.w : 0.f;
-            }
-            if (R) { const float4 t4 = *reinterpret_cast<const float4*>(R + (size_t)gm * ldr + gn); o.x += t4.x; o.y += t4.y; o.z += t4.z; o.w += t4.w; }
-            float4* dst = reinterpret_cast<float4*>(Cz + (size_t)gm * ldc + gn);
-            if (accumulate) { const float4 t4 = *dst; o.x += t4.x; o.y += t4.y; o.z += t4.z; o.w += t4.w; }
-            *dst = o;
-            if (relu_out)
-              *reinterpret_cast<float4*>(relu_out + (size_t)gm * ld_relu + gn) = make_float4(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f), fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
-          }
-        }
-      }
-      if (n_live > 0) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(acc_empty(buf)) : "memory");
-        ++at;
-      }
-    }
+    for (int k4 = 0; k4 < kBK / 8; ++k4)     // +32 bytes per k-step of 8 floats inside the swizzle row
+      gmma::mma_tf32_n128(acc, gmma::desc_sw128(sA + s * kTileBytes + a_off + k4 * 32), gmma::desc_sw128(sB + s * kTileBytes + k4 * 32),
+                          (j > 0 || k4 > 0) ? 1 : 0);
+    gmma::commit();
+    // this stage's MMAs stay in flight; the previous stage has completed and goes back to the producer
+    gmma::wait<1>();
+    if (t == 0 && j > 0) mbar_arrive(bars + 8u * (kStages + (j - 1) % kStages));
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+  gmma::wait<0>();
+  gmma::fence_regs(acc);
+  const int w = t >> 5, l = t & 31;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int gm = m0 + (wg - 1) * 64 + 16 * w + (l >> 2) + 8 * half;
+    if (gm >= M) continue;
+#pragma unroll
+    for (int c8 = 0; c8 < kBN / 8; ++c8) {
+      const int gn = n0 + 8 * c8 + 2 * (l & 3);
+      if (gn >= N) break;                                    // N % 4 == 0: gn + 1 < N as well
+      float2 o = make_float2(acc[4 * c8 + 2 * half], acc[4 * c8 + 2 * half + 1]);
+      if (bias) { const float2 t2 = *reinterpret_cast<const float2*>(bias + gn); o.x += t2.x; o.y += t2.y; }
+      if (mask) {
+        const float2 t2 = *reinterpret_cast<const float2*>(mask + (size_t)gm * ldm + gn);
+        o.x = t2.x > 0.f ? o.x : 0.f; o.y = t2.y > 0.f ? o.y : 0.f;
+      }
+      if (R) { const float2 t2 = *reinterpret_cast<const float2*>(R + (size_t)gm * ldr + gn); o.x += t2.x; o.y += t2.y; }
+      float2* dst = reinterpret_cast<float2*>(C + (size_t)gm * ldc + gn);
+      if (accumulate) { const float2 t2 = *dst; o.x += t2.x; o.y += t2.y; }
+      *dst = o;
+      if (relu_out)          // the consumer GEMM reads its A operand as stored: hand it the ReLU'd activations directly
+        *reinterpret_cast<float2*>(relu_out + (size_t)gm * ld_relu + gn) = make_float2(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
+    }
   }
 }
 
@@ -422,53 +195,6 @@ static bool encode_f32(CUtensorMap* tm, const float* base, int rows, int K, int 
 static int* g_tf32_err = nullptr;       // mapped host flag written by the watchdog
 int tf32_watchdog_flag() { return g_tf32_err ? *reinterpret_cast<volatile int*>(g_tf32_err) : 0; }
 
-// v2 launch: persistent 128 x 256 tiles (see gemm_tf32_persistent_kernel); split-K for the long-K weight-gradient shapes
-static int launch_gemm_tf32_v2(const GemmArgs& g, cudaStream_t st) {
-  CUtensorMap tmA, tmB;
-  if (!encode_f32(&tmA, g.A, g.M, g.K, g.lda) || !encode_f32(&tmB, g.B, g.N, g.K, g.ldb, tf32::k2BN)) return -1;
-  static int n_sm = 0;
-  static bool attr = false;
-  const size_t smem = (size_t)tf32::k2Stages * tf32::k2StageBytes + 1024 + 256;
-  if (!attr) {
-    cudaFuncSetAttribute(tf32::gemm_tf32_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    if (n_sm <= 0) n_sm = 148;
-    attr = true;
-  }
-  tf32::SegInfo sg;
-  sg.flags = g.seg_flags; sg.mode = g.seg_flags ? g.seg_mode : 0;
-  for (int i = 0; i < 6; ++i) sg.off[i] = g.seg_off[i];
-  const int mt = (g.M + tf32::kBM - 1) / tf32::kBM, nt = (g.N + tf32::k2BN - 1) / tf32::k2BN;
-  const int tiles = mt * nt;
-  int splits = 1, k_per = g.K;
-  if (g.splitk_ws && !g.bias && !g.mask && !g.R && !g.relu_out && tiles < n_sm / 2 && g.K >= 1024) {
-    splits = (n_sm + tiles - 1) / tiles;
-    if (splits > 32) splits = 32;
-    while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
-    if (splits > 1) {
-      k_per = ((g.K + splits - 1) / splits + tf32::kBK - 1) / tf32::kBK * tf32::kBK;
-      splits = (g.K + k_per - 1) / k_per;
-    }
-  }
-  const int total = tiles * splits;
-  const int grid = total < n_sm ? total : n_sm;
-  if (splits > 1) {
-    tf32::gemm_tf32_persistent_kernel<<<grid, tf32::kThreads, smem, st>>>(tmA, tmB, g.splitk_ws, g.N, g.M, g.N, g.K, nullptr, nullptr, 0, nullptr,
-                                                                          0, 0, k_per, splits, g.skip_if_zero, sg, g_tf32_err, nullptr, 0);
-    tf32::splitk_reduce_kernel<<<(g.M * g.N + 255) / 256, 256, 0, st>>>(g.splitk_ws, splits, g.C, g.ldc, g.M, g.N, g.accumulate,
-                                                                        g.skip_if_zero, sg);
-    launch_counter() += 2;
-  } else {
-    ++launch_counter();
-    tf32::gemm_tf32_persistent_kernel<<<grid, tf32::kThreads, smem, st>>>(tmA, tmB, g.C, g.ldc, g.M, g.N, g.K, g.bias, g.mask, g.ldm, g.R, g.ldr,
-                                                                          g.accumulate, g.K, 1, g.skip_if_zero, sg, g_tf32_err, g.relu_out,
-                                                                          g.ld_relu);
-  }
-  return 0;
-}
-
 // Only the NT layout with un-transformed operands (at=false, bt=true, no relu_a / relu_b).  Returns 0, or -1 when the
 // shape cannot go through TMA (unaligned rows) -- the caller then falls back to launch_gemm.
 int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st) {
@@ -481,15 +207,10 @@ int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st) {
     int* h = nullptr;
     if (cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped) == cudaSuccess) { *h = 0; cudaHostGetDevicePointer(&g_tf32_err, h, 0); }
   }
-  // The persistent 128 x 256 kernel is opt-in (SRF_TF32_V2=1): on the training step it is faster on the forward shapes (4.0 vs 4.5 ms)
-  // but slower on the weight-gradient shapes, whose few large tiles quantise badly over 148 one-CTA SMs (8.6 vs 7.9 ms): 12.7 vs 12.5 ms
-  // per step in total (profiles/r2_history.md).
-  static const bool use_v2 = getenv("SRF_TF32_V2") != nullptr;
-  if (use_v2 && g.N >= 64) return launch_gemm_tf32_v2(g, st);
   CUtensorMap tmA, tmB;
   if (!encode_f32(&tmA, g.A, g.M, g.K, g.lda) || !encode_f32(&tmB, g.B, g.N, g.K, g.ldb)) return -1;
   static bool attr = false;
-  const size_t smem = 2 * tf32::kStages * tf32::kTileBytes + 1024 + 256;
+  const size_t smem = 2 * tf32::kStages * tf32::kTileBytes + 1024 + 64;
   if (!attr) { cudaFuncSetAttribute(tf32::gemm_tf32_nt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
   dim3 grid((g.N + tf32::kBN - 1) / tf32::kBN, (g.M + tf32::kBM - 1) / tf32::kBM);
   tf32::SegInfo sg;
@@ -498,7 +219,7 @@ int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st) {
   const int tiles = grid.x * grid.y;
   int splits = 1;
   if (g.splitk_ws && !g.bias && !g.mask && !g.R && !g.relu_out && tiles < 96 && g.K >= 1024) {
-    splits = (2 * 148 + tiles - 1) / tiles;
+    splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
     if (splits > 32) splits = 32;
     while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
   }

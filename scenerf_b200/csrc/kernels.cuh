@@ -55,11 +55,13 @@ struct GemmArgs {
   float* relu_out = nullptr; int ld_relu = 0;   // tf32 kernel only: the epilogue also stores max(result, 0) here (the next GEMM's A operand)
 };
 int launch_gemm(const GemmArgs& g, cudaStream_t st);
+// SM count of the current device (cached; 132 on an H100 SXM): sizes waves, split-K factors and point chunks
+int device_sm_count();
 // per-thread count of kernels launched by the float32 / tf32 MLP paths (gemm.cu, gemm_tf32.cu, mlp_simt.cu, backward.cu);
 // the run_* entry points report the difference as their launch count (srf_last_launch_count)
 int& launch_counter();    // 0, or -1 for an operand-layout combination that is not instantiated
 
-// gemm_tf32.cu : the same contract on tensor cores (tcgen05 kind::tf32, float32 operands read in place); NT layout only
+// gemm_tf32.cu : the same contract on tensor cores (wgmma .tf32, float32 operands read in place); NT layout only
 // (at=false, bt=true, no operand ReLU).  Returns 0, or -1 when the shape cannot be expressed as TMA tensor maps.
 int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st);
 int tf32_watchdog_flag();
@@ -88,7 +90,7 @@ void launch_ray_backward(const DevParams& p, int R, const float* raw, const floa
                          const float* gauss_raw, const float* noise_n, const srf_outputs& fwd, const srf_outputs& cot,
                          float* graw_main, float* graw_gauss, cudaStream_t st);
 
-// mlp_tc.cu : tcgen05 tensor-core point MLP.
+// mlp_tc.cu : wgmma tensor-core point MLP.
 //   split != 0: the fp32-grade layout (hi + lo fp16 images of W 2^s, see mlp_tc.cu) read through w.tc_split_packed
 size_t tc_weights_bytes(int d_out, int d_latent, int split);
 int pack_weights_tc(const srf_mlp_weights& w, void* dst, size_t bytes, int split, cudaStream_t st);
@@ -99,7 +101,7 @@ int run_point_mlp_tc(const DevParams& p, const srf_mlp_weights& w, const float* 
                      int n_per, float* raw_out, int32_t* dbg_sphere, int flags, void* workspace, size_t ws_bytes,
                      cudaStream_t st);
 
-// conv_tf32.cu : the spherical decoder's 3x3 (dilated) convolutions as a tcgen05 kind::tf32 implicit GEMM on channels-last maps
+// conv_tf32.cu : the spherical decoder's 3x3 (dilated) convolutions as a wgmma .tf32 implicit GEMM on channels-last maps
 //   (unet2d_sphere.py:9-57) + the UpSampleBN front end (bilinear align_corners=True upsample of the coarser map, concat with the skip map)
 int launch_conv3x3_tf32(const float* in, int H, int W, int Cin, const float* w9, int Cout, int dil, const float* scale, const float* shift,
                         const float* residual, int ld_res, float slope, int round_out, float* out32, int ld32, void* out16, int ld16,
@@ -118,7 +120,7 @@ int run_preproject(const DevParams& p, const srf_mlp_weights& w, int fp16, void*
 // non-zero after the kernel's mbarrier watchdog fired: 0x40000000 | warp<<24 | (barrier smem offset)<<4 | parity
 int tc_watchdog_flag();
 // diagnostic: stop every tile after `debug_layer` (1,2,4,5,7,8,9,10 -- see the tile program in mlp_tc.cu) and dump the
-// raw fp32 accumulator (n_tiles*128, 512) to debug_acc
+// raw fp32 accumulator (n_tiles*64, 512) to debug_acc
 int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n,
                            int n_per, float* raw_out, int32_t* dbg_sphere, int flags, void* workspace, size_t ws_bytes,
                            int debug_layer, float* debug_acc, cudaStream_t st);

@@ -9,7 +9,10 @@
 
 namespace srf {
 
-constexpr int kChunk = 9472;                  // points per pass: 74 row tiles x 4 column tiles = 296 CTAs = 148 SMs x 2 (x_in chunk 96 MB)
+// points per pass: one wave of 2 CTAs per SM of the GEMM chain's 128 x 128 tiles (4 column tiles of the 512-wide layers)
+// -> 66 row tiles = 8448 points = 264 CTAs on the 132 SMs of an H100 SXM (x_in chunk 86 MB)
+static int simt_chunk() { return (2 * device_sm_count() / 4 > 0 ? 2 * device_sm_count() / 4 : 1) * 128; }
+#define kChunk (simt_chunk())
 
 static inline int xin_ld(int d_latent) { return ((d_latent + kDX + 31) / 32) * 32; }
 

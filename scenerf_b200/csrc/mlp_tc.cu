@@ -1,13 +1,14 @@
-// Fused point-MLP on Blackwell tensor cores (sm_100a): one persistent, warp-specialised kernel does, per 128-point
-// tile, projection -> integer sphere coords -> positional encoding -> 5-scale bilinear gather -> the whole ResnetFC
-// (lin_in, 3 x [lin_z, fc_0, fc_1], lin_out) with tcgen05.mma (fp16 operands, fp32 accumulators in TMEM).  The
-// (N x 2522) x_in matrix of the reference (scenerf/models/scenerf.py:527-531) and all hidden activations never touch
-// HBM: gathered features / activations are produced straight into 128B-swizzled shared-memory A tiles, weights are
-// streamed as pre-swizzled stage images by cp.async.bulk (TMA engine, UBLKCP) through an mbarrier ring.
+// Fused point-MLP on Hopper tensor cores (sm_90a): one persistent kernel does, per 64-row tile, projection -> integer
+// sphere coords -> positional encoding -> 5-scale bilinear gather -> the whole ResnetFC (lin_in, 3 x [lin_z, fc_0, fc_1],
+// lin_out) with wgmma (fp16 operands, fp32 accumulators in registers).  The (N x 2522) x_in matrix of the reference
+// (scenerf/models/scenerf.py:527-531) and all hidden activations never touch HBM: gathered features / activations are
+// produced straight into 128B-swizzled shared-memory A tiles, weights are streamed as pre-swizzled stage images by
+// cp.async.bulk (TMA engine) through an mbarrier ring.
 //
 // Reference computed here: scenerf.py:505-531 (predict up to mlp(x_in)), resnetfc.py:54-63,133-164.
 //
-// Tile program (A-chunk = 128 rows x 64 k, fp16, K-major SW128; each A chunk meets 4 B images of 128 rows(N) x 64 k):
+// Tile program (A chunk = 64 rows x 64 k, fp16, K-major SW128; each A chunk meets the 128 x 64 weight images of the
+// warpgroup's two N-quarters):
 //   L0  lin_in   1 chunk   fresh   ACC  = x Win^T
 //   L1  lin_z0   KZ chunks acc     ACC += z Wz0^T                  -> E1: h = ACC + c0            ; A = relu(h)
 //   L2  fc_0     8 chunks  fresh   ACC  = relu(h) W0^T             -> E2: net = ACC + b0          ; A = relu(net)
@@ -16,19 +17,22 @@
 //   ... (blocks 1, 2) ...
 //   L9  fc_1     8         fresh                                   -> E3: h = h + ACC + b1_2      ; A = relu(h)
 //   L10 lin_out  8 (N=16)  fresh   ACC[:, :16] = relu(h) Wout^T    -> E4: out = ACC + bout
-// The fp32 hidden state h (128 x 512) cannot share the 512 TMEM columns with the accumulator of the next layer, so
-// it lives in a per-CTA 256 KB scratch that stays L2-resident (9 B/cycle/SM of traffic); biases are folded into the
-// epilogues as cumulative vectors c_b.
+// Biases are folded into the epilogues as cumulative vectors c_b.
 //
-// Warp roles (320 threads, 1 CTA / SM):  warp 0 = weight producer (bulk copies), warp 1 = MMA issuer + TMEM owner,
-// warps 2..9 = 256 workers: geometry front-end, A-chunk producers (gather / activations) and TMEM epilogues.
+// Threads: two warpgroups (256 threads, 1 CTA / SM).  Warpgroup g owns output columns [256 g, 256 g + 256) of every
+// 512-wide layer as two 64 x 128 register accumulators (wgmma m64n128k16), streams ITS weight images through its own
+// ring (one thread issues the bulk copies, running a ring's depth ahead of its MMAs), and runs the epilogues of its
+// columns from registers.  Both warpgroups produce the shared A tiles together: geometry, positional encoding, the
+// latent gather (overlapping the MMAs of the previous latent chunk) and the activations written by the epilogues.
+// The fp32 hidden state h (64 x 512) does not fit next to the accumulators: it lives in a per-CTA scratch that stays
+// L2-resident, in the accumulator's register order (each thread reads back exactly what it wrote).
 //
-// CTA pairs (template CG = 2, the default): two CTAs of a 2-cluster run `tcgen05.mma.cta_group::2` with M = 256 --
-// each CTA owns a 128-point tile (its own A tiles, its own 128 TMEM lanes) but stages only HALF of every weight tile
-// (N = 256 per MMA, 128 rows per CTA), which halves the bytes every SM has to pull from L2 per FLOP.  Only the
-// leader CTA (rank 0) issues MMAs; the peer's workers arrive remotely on the leader's A-full barriers, the peer's
-// warp 1 relays its weight-full barriers to the leader, and the leader's tcgen05.commit multicasts the "empty" /
-// "accumulator complete" signals to both CTAs.  CG = 1 is the single-CTA variant (M = 128, N = 128).
+// Split (fp32-grade) mode: every fp32 operand x is carried as fp16 hi = rn(x) and lo = rn(x - hi).  The A tile stacks
+// the two parts of 32 points as ROWS (rows 0-31 hi, rows 32-63 lo -- MMA rows are independent), every weight image is
+// followed by the image of its low parts and both are accumulated into the same registers:
+//   D[r] = x_hi (W_hi + W_lo)^T ,  D[r+32] = x_lo (W_hi + W_lo)^T ,  result[r] = D[r] + D[r+32]   (epilogue)
+// Row r + 32 sits in the thread 64 above the thread of row r, at the same register index: the epilogue hands those
+// partial sums over through the per-CTA scratch.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -36,38 +40,40 @@
 #include <cstring>
 #include <type_traits>
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace srf {
 namespace tc {
 
-constexpr int kTileM = 128;
+constexpr int kTileM = 64;                        // MMA rows per tile (points: 64, split mode 32)
 constexpr int kChunkK = 64;                       // fp16 elements per A/B row = 128 bytes = one SW128 atom row
-constexpr int kASlots = 8, kASlotBytes = kTileM * 128;          // 16 KB
-constexpr int kBSlots = 6, kBRows = 128, kBSlotBytes = kBRows * 128;   // 16 KB
+constexpr int kAChunkBytes = kTileM * 128;        // 8 KB
+constexpr int kBRows = 128, kBSlotBytes = kBRows * 128;   // one weight image: 128 rows (N) x 64 k = 16 KB
 constexpr int kHiddenChunks = kHidden / kChunkK;  // 8
 constexpr int kQuarters = kHidden / kBRows;       // 4 N-quarters of 128
-constexpr int kOutN = 16;                         // lin_out padded to the minimum UMMA N for M=128
+constexpr int kOutN = 16;                         // lin_out padded to N = 16
 constexpr int kOutImgBytes = kOutN * 128;         // 2 KB
-constexpr int kWorkerWarps = 8, kWorkerThreads = kWorkerWarps * 32;
-constexpr int kThreads = 64 + kWorkerThreads;     // 320
-constexpr int kTmemCols = 512;
+constexpr int kThreads = 256;                     // two warpgroups
 constexpr int kNumBias = 8;                       // c0,c1,c2, b_fc0[0..2], b_fc1_2, b_out(padded)
 constexpr size_t kHeaderBytes = (size_t)kNumBias * kHidden * sizeof(float);   // 16 KB
 constexpr int kNumLayers = 11;
 // split-mode blobs: the power-of-two weight scale 2^s and its inverse live in unused entries of the b_out header row
 constexpr int kScaleSlot = 7 * kHidden + 256, kInvScaleSlot = 7 * kHidden + 257;
+// per-CTA scratch (floats): fp32 hidden state (2 warpgroups x 2 quarters x 64 registers x 128 threads), then the
+// split-mode hand-over of the low-part sums (2 x 2 x 64 x 64)
+constexpr size_t kScratchFloats = (size_t)2 * kTileM * kHidden;   // 256 KB per CTA
+constexpr size_t kExchangeOffset = (size_t)2 * 2 * 64 * 128;
 
 // dynamic shared memory carve-up
-constexpr int kSmemA = 0;
-constexpr int kSmemB = kSmemA + kASlots * kASlotBytes;                 // 131072
-constexpr int kSmemBar = kSmemB + kBSlots * kBSlotBytes;               // 229376
-constexpr int kZCache = 4;                        // latent chunks cached across the three lin_z passes (fine scales)
-constexpr int kNumBars = 2 * kASlots + 2 * kBSlots + 3 + 4;            // a_full/empty, b_full/empty, half_full[2], meta, zbar[4]
-constexpr int kSmemTmemPtr = kSmemBar + kNumBars * 8;
-constexpr int kSmemMask = kSmemTmemPtr + 8;                            // 2 x uint64 active-chunk masks (double buffer)
-constexpr int kSmemSph = kSmemMask + 16;                               // 2 x short2 (sx,sy) per row: current + next tile
-constexpr int kSmemLayerRow = kSmemSph + 2 * kTileM * 4;              // kNumLayers x uint32: first image row of every layer (producer)
-constexpr int kSmemTotal = kSmemLayerRow + 48;
+constexpr int kSmemAct = 0;                                            // 8 A chunks: activations of the current layer
+constexpr int kSmemX = kSmemAct + kHiddenChunks * kAChunkBytes;        // x chunk (positional encoding | view direction)
+constexpr int kSmemZ = kSmemX + kAChunkBytes;                          // 2 latent chunks (double buffer)
+constexpr int kRingBytes = 4 * kBSlotBytes;                            // per warpgroup: 4 fp16 images or 2 hi/lo pairs
+constexpr int kSmemRing = kSmemZ + 2 * kAChunkBytes;
+constexpr int kSmemBar = kSmemRing + 2 * kRingBytes;                   // full[2][4]
+constexpr int kSmemSph = kSmemBar + 2 * 4 * 8;                         // short2 (sx,sy) per point
+constexpr int kSmemMask = kSmemSph + kTileM * 4;                       // active latent chunks of the tile
+constexpr int kSmemTotal = kSmemMask + 16;
 static_assert(kSmemTotal + 1024 <= 232448, "shared memory budget");
 
 struct Layer { int chunks_is_kz, chunks, fresh, signal, is_out; };
@@ -84,22 +90,18 @@ struct KernelArgs {
   const float* viewdir;    // (n/n_per,3)
   int n, n_per, n_tiles, kz;
   const unsigned char* wblob;   // header (biases) + stage images
-  float* scratch;          // gridDim.x * 128*512 floats
+  float* scratch;          // gridDim.x * kScratchFloats
   float* raw_out;          // (n, d_out)
   int d_out;
   int32_t* dbg_sphere;     // (n,2) or null
   int skip_zero;           // SRF_FLAG_SKIP_ZERO_CHUNKS
-  int hidden_fp16;         // SRF_FLAG_HIDDEN_FP16: the hidden state travels between blocks as fp16 (scratch bytes halved)
-  int split;               // fp32-grade mode: 64 points per tile, A rows 0-63 = fp16 hi parts, rows 64-127 = lo parts; hi+lo weight images
+  int hidden_fp16;         // SRF_FLAG_HIDDEN_FP16: the hidden state travels between blocks as fp16
   const unsigned char* preproj;  // pre-projected latent table (preproj.cu) or null: rows of 3 x 512 values (fp16 in fp16 mode, fp32 in
                                  // split mode); when set, the lin_z GEMMs are not executed and E1 adds the row of the point's sphere pixel
   int pre_W1, pre_H1;      // sphere_W + 1, sphere_H + 1: row = sy * pre_W1 + sx inside, pre_W1 * pre_H1 (the zero row) outside
-  int use_tmap;            // CTA pairs: weight images by cp.async.bulk.tensor.cta_group::2 that signals the LEADER's barrier
   int debug_layer;         // -1, or: stop every tile after this layer's ACC is complete and dump it
-  float* debug_acc;        // (n_tiles*128, 512)
-  unsigned char* zcache;   // gridDim.x * kZCache * 16 KB: gathered latent chunks 0..kZCache-1 of the current tile
+  float* debug_acc;        // (n_tiles*64, 512)
   int* error_flag;         // set to non-zero by the watchdog
-  unsigned long long* prof; // optional (SRF_TC_PROF=1): per-CTA cycle counters, 16 per CTA
 };
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -109,9 +111,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -133,8 +132,6 @@ __device__ __noinline__ void mbar_timeout(int* error_flag, uint32_t bar, uint32_
   __threadfence_system();
   __trap();
 }
-// The spin loop lives out of line: the tile program has ~170 wait sites and each inlined loop (clock reads, 64-bit compare,
-// watchdog call) was ~25 instructions -- a fifth of the kernel's code for a path that only runs while there is nothing to do.
 __device__ __noinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity, int* error_flag) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
@@ -147,8 +144,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* er
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // The 2 x 10.9 MB of weight images are re-read by every CTA for every tile while the feature pyramid streams through
 // L2 once per frame: ask L2 to keep the weights (evict_last) so that the stream sees L2-hit latency.
@@ -162,138 +157,14 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar), "l"(policy)
                : "memory");
 }
-
-// 2-D tiled TMA load whose mbarrier may live in the peer CTA of the pair (cta_group::2): both CTAs of a pair issue it
-// with their own shared-memory destination and the LEADER's barrier, so the MMA issuer waits on one barrier for both
-// halves of a weight tile (no relay hop).  c0 = element column, c1 = row of the [rows x 64] fp16 image tensor.
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst_smem, const void* tmap, int c0, int c1, uint32_t mbar_cluster,
-                                                 uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(mbar_cluster), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_addr` in CTA `rank` of this cluster
-__device__ __forceinline__ uint32_t map_to_cta(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  // default .release.cta semantics: the data this guards was already handed to the async proxy by
-  // fence.proxy.async; a .release.cluster here compiles to MEMBAR.ALL.GPU and drains every global store first
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void atom_or_remote_u64(uint32_t cluster_addr, unsigned long long v) {
-  asm volatile("red.relaxed.cluster.shared::cluster.or.b64 [%0], %1;" ::"r"(cluster_addr), "l"(v) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// wait on a barrier that CTAs of the cluster arrive on remotely (acquire at cluster scope)
-__device__ __noinline__ void mbar_wait_cluster_spin(uint32_t bar, uint32_t parity, int* error_flag) {
-  const long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) mbar_timeout(error_flag, bar, parity);
-  }
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, int* error_flag) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  mbar_wait_cluster_spin(bar, parity, error_flag);
-}
-
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  if constexpr (CG == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-  else asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::f16.  CG=2: issued by the leader CTA for the pair (M=256, each CTA
-// contributes its own A tile and half of the B rows, found at the same shared-memory offsets in both CTAs).
-template <int CG>
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed; CG=2: the arrive is
-// delivered to the barrier at this offset in BOTH CTAs of the pair
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CG == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-  } else {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(mask)
-                 : "memory");
-  }
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  // no "memory" clobber on purpose: global loads of the next item may be hoisted above this store (volatile asm
-  // statements still keep their order relative to the fences / arrives that publish the tile)
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d));
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
 }
 // {relu(lo), relu(hi)} -> packed fp16x2 in one instruction (the ReLU of the reference rides on the conversion)
 __device__ __forceinline__ uint32_t pack_relu_half2(float lo, float hi) {
@@ -305,11 +176,6 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
 // split mode: (a, b) -> packed fp16 high parts rn(x) and packed low parts rn(x - rn(x)); hi + lo carries 22 mantissa
 // bits (the low part goes subnormal below |x| ~ 2^-3, absolute error <= 2^-25 there)
 __device__ __forceinline__ void split_half2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -320,38 +186,8 @@ __device__ __forceinline__ void split_half2(float a, float b, uint32_t& hi, uint
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout): start address >> 4 in
-// bits [0,14), leading byte offset (unused for swizzled K-major, =1) in [16,30), stride byte offset (1024 B between
-// 8-row core groups) in [32,46), descriptor version 1 in [46,48), layout type 2 (SWIZZLE_128B) in [61,64).
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) at [4,6), a/b format F16 (0) at [7,10) and
-// [10,13), a/b K-major (0) at 15/16, N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
 // byte offset of (row, 16-byte granule g) inside a 128B-swizzled K-major tile whose rows are 128 bytes
 __device__ __forceinline__ uint32_t sw128_offset(int row, int g) { return (uint32_t)(row * 128 + ((g ^ (row & 7)) << 4)); }
-
-// ---------------------------------------------------------------------------------------------------------------
-// Ring bookkeeping shared by all roles (every role walks the same program, so (slot, parity) stay in lock-step).
-// ---------------------------------------------------------------------------------------------------------------
-struct Ring {
-  int slot = 0;
-  uint32_t phase = 0;
-  template <int N>
-  __device__ __forceinline__ void advance() {
-    if (++slot == N) { slot = 0; phase ^= 1; }
-  }
-};
 
 __device__ __forceinline__ int layer_chunks(int l, int kz) { return kLayers[l].chunks_is_kz ? kz : kLayers[l].chunks; }
 // chunk c of a lin_z layer is active for this tile?  (mask bit c; all ones when skipping is off)
@@ -368,54 +204,6 @@ __device__ __forceinline__ uint64_t chunk_mask_for_scales(const DevParams& p, ui
   return m;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Tile program walker: the ONE definition of the order in which MMAs (and therefore weight images and A chunks) are
-// consumed.  The weight producer, the weight-full relay and the MMA issuer all walk it with their own visitor, so
-// they cannot disagree.
-//
-//   T0      lin_in (1 chunk) + lin_z0 (kz chunks), K-outer, both accumulator halves          -> EV_ALL
-//   fc_0 b  four S-groups of the 512x512 layer:  S1 (k0-3, half 0)  S2 (k0-3, half 1) -> EV_BANK0_FREE
-//                                                S3 (k4-7, half 0) -> EV_HALF0    S4 (k4-7, half 1) -> EV_BANK1_FREE, EV_HALF1
-//   fc_1 b  S1 S2 | lin_z(b+1) K-outer (accumulates into both halves) | S3 S4   (same events)
-//   lin_out 8 chunks, N = 16                                                                  -> EV_OUT
-// Accumulator half 0 of a layer is complete after S3 and half 1 after S4, so the epilogue of half 0 overlaps the
-// MMAs of S4 and the epilogue of half 1 overlaps S1 of the next layer (which only touches half 0 and A chunks 0-3).
-// ---------------------------------------------------------------------------------------------------------------
-enum OpKind { OP_KOUTER = 0, OP_SGROUP = 1, OP_OUT = 2 };
-enum EvKind { EV_ALL = 0, EV_BANK0_FREE = 1, EV_HALF0 = 2, EV_BANK1_FREE_HALF1 = 3, EV_OUT = 4, EV_PRE_S1 = 5, EV_PRE_S2 = 6 };
-
-template <class V>
-__device__ __forceinline__ void walk_tile(int kz, uint64_t mask, int last_layer, V& v) {
-  // T0
-  v.op(OP_KOUTER, 0, 0, 0, /*fresh*/ 1);
-  for (int c = 0; c < kz; ++c)
-    if ((mask >> c) & 1ull) v.op(OP_KOUTER, 1, c, 0, 0);
-  v.ev(EV_ALL);
-  if (last_layer == 1) return;
-  for (int b = 0; b < SRF_NUM_BLOCKS; ++b) {
-    for (int which = 0; which < 2; ++which) {               // 0: fc_0, 1: fc_1
-      const int l = 2 + 3 * b + which;
-      v.ev(EV_PRE_S1);
-      for (int k = 0; k < 4; ++k) v.op(OP_SGROUP, l, k, 0, k == 0);
-      v.ev(EV_PRE_S2);
-      for (int k = 0; k < 4; ++k) v.op(OP_SGROUP, l, k, 1, k == 0);
-      v.ev(EV_BANK0_FREE);
-      if (which == 1 && b < SRF_NUM_BLOCKS - 1) {
-        for (int c = 0; c < kz; ++c)
-          if ((mask >> c) & 1ull) v.op(OP_KOUTER, 4 + 3 * b, c, 0, 0);
-      }
-      for (int k = 4; k < 8; ++k) v.op(OP_SGROUP, l, k, 0, 0);
-      v.ev(EV_HALF0);
-      for (int k = 4; k < 8; ++k) v.op(OP_SGROUP, l, k, 1, 0);
-      v.ev(EV_BANK1_FREE_HALF1);
-      const int done_layer = (which == 0) ? l : ((b < SRF_NUM_BLOCKS - 1) ? 4 + 3 * b : 9);
-      if (last_layer == done_layer) return;
-    }
-  }
-  for (int k = 0; k < 8; ++k) v.op(OP_OUT, 10, k, 0, k == 0);
-  v.ev(EV_OUT);
-}
-
 // byte offset of the first image of chunk k of layer l inside the image region of the blob
 //   parts = 1 (fp16 images) or 2 (split mode: every image is followed by the image of the fp16 low parts)
 __device__ __forceinline__ size_t chunk_image_offset(int l, int k, int kz, int parts) {
@@ -425,1019 +213,515 @@ __device__ __forceinline__ size_t chunk_image_offset(int l, int k, int kz, int p
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Weight stream of one warpgroup.  A stage ("slot") is, for a 512-wide layer, chunk k of one of the warpgroup's two
+// N-quarters (hi + lo images in split mode: contiguous in the blob); for lin_out, the 16 x 64 image(s) of chunk k
+// (warpgroup 0 only).  The order is the tile program's order; lin_z chunks not in the tile's mask are skipped.
+// ---------------------------------------------------------------------------------------------------------------
+struct Cursor {
+  int l = 0, k = 0, j = 0;
+  // move to the first slot at or after (l, k, j) that exists; false when the tile's stream is exhausted
+  __device__ __forceinline__ bool normalize(int kz, uint64_t mask, int last_layer, int wg) {
+    while (l <= last_layer) {
+      if (l == kNumLayers - 1 && wg != 0) return false;
+      if (j >= (kLayers[l].is_out ? 1 : 2)) { j = 0; ++k; }
+      if (k >= layer_chunks(l, kz)) { k = 0; ++l; continue; }
+      if (!chunk_active(l, k, mask)) { ++k; continue; }
+      return true;
+    }
+    return false;
+  }
+};
+
+// next active latent chunk of lin_z layer l after chunk c (-1: none)
+__device__ __forceinline__ int next_active(int kz, uint64_t mask, int c) {
+  for (++c; c < kz; ++c)
+    if ((mask >> c) & 1ull) return c;
+  return -1;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------------------------
 // PRE: the latent-table variant (a.preproj set): no lin_z chunk exists in the tile program and the E1 epilogues add table rows.
-// A template parameter so that the dense kernels carry none of that code (it cost them 3-5 % as a runtime branch).
-template <int CG, bool PROF, bool H16, bool SPLIT, bool PRE>
+template <bool H16, bool SPLIT, bool PRE>
 __global__ void __launch_bounds__(kThreads, 1)
-point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__ KernelArgs a,
-                    const __grid_constant__ CUtensorMap tm_main, const __grid_constant__ CUtensorMap tm_out) {
+point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__ KernelArgs a) {
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   // SWIZZLE_128B tiles need 1024-byte alignment; the launch reserves 1 KB of slack for this round-up
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   const uint32_t smem_base = smem_u32(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar0 = smem_base + kSmemBar;
-  auto a_full = [&](int s) { return bar0 + 8u * s; };
-  auto a_empty = [&](int s) { return bar0 + 8u * (kASlots + s); };
-  auto b_full = [&](int s) { return bar0 + 8u * (2 * kASlots + s); };
-  auto b_empty = [&](int s) { return bar0 + 8u * (2 * kASlots + kBSlots + s); };
-  auto half_full = [&](int h) { return bar0 + 8u * (2 * kASlots + 2 * kBSlots + h); };
-  const uint32_t meta_full = bar0 + 8u * (2 * kASlots + 2 * kBSlots + 2);
-  auto zbar = [&](int s) { return bar0 + 8u * (2 * kASlots + 2 * kBSlots + 3 + s); };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + kSmemTmemPtr);
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, t = tid & 127, w = t >> 5, lane = tid & 31;
+  constexpr int kParts = SPLIT ? 2 : 1;                 // weight images per (chunk, quarter): hi (+ lo)
+  constexpr int kPts = SPLIT ? kTileM / 2 : kTileM;     // points per tile
+  constexpr int kSlotBytes = kBSlotBytes * kParts;
+  constexpr int kSlots = kRingBytes / kSlotBytes;       // 4 (fp16) or 2 (split)
+  const uint32_t ring = smem_base + kSmemRing + (uint32_t)wg * kRingBytes;
+  auto full_bar = [&](int s) { return smem_base + kSmemBar + 8u * (uint32_t)(wg * 4 + s); };
+  short2* sph_smem = reinterpret_cast<short2*>(smem + kSmemSph);
   volatile unsigned long long* mask_smem = reinterpret_cast<volatile unsigned long long*>(smem + kSmemMask);
-  short2* sph_smem = reinterpret_cast<short2*>(smem + kSmemSph);   // [2][128]
 
-  const uint32_t crank = (CG == 2) ? cluster_ctarank() : 0u;     // 0 = leader of the pair
-  const bool leader = (crank == 0);
-  if (threadIdx.x == 0) {
-    // A-full: every worker warp of every CTA of the group arrives (on the leader's barrier)
-    for (int s = 0; s < kASlots; ++s) { mbar_init(a_full(s), kWorkerWarps * CG); mbar_init(a_empty(s), 1); }
-    // B-full: the local producer's arrive.expect_tx (+ its bytes); on the leader of a pair also the peer's relay
-    //         (with tensor-map loads both CTAs' bytes complete on the leader's barrier instead: one arrival)
-    for (int s = 0; s < kBSlots; ++s) { mbar_init(b_full(s), (CG == 2 && leader && !a.use_tmap) ? 2 : 1); mbar_init(b_empty(s), 1); }
-    mbar_init(half_full(0), 1);
-    mbar_init(half_full(1), 1);
-    mbar_init(meta_full, kWorkerWarps);
-    for (int s = 0; s < 4; ++s) mbar_init(zbar(s), 1);
-    mask_smem[0] = 0ull; mask_smem[1] = 0ull;
-    // row (128-byte unit) of the first weight image of every layer inside the image region: the producer looks images up per op,
-    // and summing the layer sizes there cost it ~80 instructions per image -- on the one thread that has to keep the ring full
-    for (int l = 0; l < kNumLayers; ++l)
-      reinterpret_cast<volatile uint32_t*>(smem + kSmemLayerRow)[l] = (uint32_t)(chunk_image_offset(l, 0, a.kz, SPLIT ? 2 : 1) / 128);
+  if (tid == 0) {
+    for (int s = 0; s < 8; ++s) mbar_init(smem_base + kSmemBar + 8u * s, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<CG>(smem_base + kSmemTmemPtr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  if (CG == 2) cluster_sync_all();           // the peer must not arrive on uninitialised barriers
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // tiles: CTA group g handles tile groups g, g+n_cgroups, ...; CTA `crank` takes tile group*CG + crank.  Both CTAs
-  // of a pair run the same number of tiles (a tile index >= n_tiles is a dummy with no valid rows).
-  const int n_cgroups = gridDim.x / CG, cgroup_id = blockIdx.x / CG;
-  const int n_groups = (a.n_tiles + CG - 1) / CG;
 
   const int kz = a.kz;
   const int last_layer = (a.debug_layer >= 0) ? a.debug_layer : (kNumLayers - 1);
   const unsigned char* images = a.wblob + kHeaderBytes;
-  constexpr int kMmaN = kBRows * CG;                    // N of one MMA (128 rows from each CTA of the group)
-  constexpr int kHalves = kQuarters / CG;               // accumulator column groups of kMmaN: 2 halves (pairs) or 4 quarters
-  // Split (fp32-grade) mode: every fp32 operand x is carried as fp16 hi = rn(x) and lo = rn(x - hi).  The A tile
-  // stacks the two parts of 64 points as ROWS (rows 0-63 hi, rows 64-127 lo -- MMA rows are independent), every
-  // weight image is followed by the image of its low parts and both are accumulated into the same TMEM columns:
-  //   D[r]    = x_hi (W_hi + W_lo)^T ,  D[r+64] = x_lo (W_hi + W_lo)^T ,  result[r] = D[r] + D[r+64]   (epilogue)
-  // i.e. all four partial products with fp32 accumulation, 2 MMAs per 64 points instead of 1 per 128.
-  constexpr int kParts = SPLIT ? 2 : 1;                 // weight images per (chunk, quarter): hi (+ lo)
-  constexpr int kPts = SPLIT ? kTileM / 2 : kTileM;     // points per tile
+  const float* bias = reinterpret_cast<const float*>(a.wblob);
+  float* scratch = a.scratch + (size_t)blockIdx.x * kScratchFloats;
+  float* hbuf = scratch + (size_t)wg * (2 * 64 * 128);             // [j][reg][thread] of this warpgroup
+  float* xbuf = scratch + kExchangeOffset + (size_t)wg * (2 * 64 * 64);   // split: [j][reg][hi thread]
+  const uint64_t policy = l2_policy_evict_last();
 
-  // ---- visitor pieces shared by producer and relay: which weight images does an op need from THIS CTA? ----------
-  //   OP_KOUTER: all column groups of chunk k  -> kHalves images (quarter i*CG + crank)
-  //   OP_SGROUP: one half h of chunk k.  CG=2: 1 image (quarter 2h + crank); CG=1: 2 images (quarters 2h, 2h+1)
-  //   OP_OUT:    the [16 x 64] image, 1/CG of it per CTA
-  if (warp == 0) {
-    // ===================================== weight producer =====================================================
-    if (lane == 0) {
-      struct Producer {
-        const unsigned char* images; uint32_t smem_base, bar0; int kz; uint32_t crank; int* err; Ring rb; uint64_t policy;
-        const CUtensorMap* tmm; const CUtensorMap* tmo; bool use_tmap; const volatile uint32_t* layer_row;
-        __device__ __forceinline__ uint32_t bfull(int s) const { return bar0 + 8u * (2 * kASlots + s); }
-        __device__ __forceinline__ uint32_t bempty(int s) const { return bar0 + 8u * (2 * kASlots + kBSlots + s); }
-        __device__ __forceinline__ void load(const unsigned char* src, uint32_t bytes) {
-          mbar_wait(bempty(rb.slot), rb.phase ^ 1, err);
-          mbar_arrive_expect_tx(bfull(rb.slot), bytes);
-          bulk_g2s(smem_base + kSmemB + rb.slot * kBSlotBytes, src, bytes, bfull(rb.slot), policy);
-          rb.advance<kBSlots>();
+  // ---- weight stream: producer (thread 0 of the warpgroup) and consumer positions -----------------------------
+  Cursor pc;
+  bool p_live = false;
+  uint32_t ppos = 0, cpos = 0, done = 0;                // slots issued / consumed / known complete (whole kernel)
+  uint64_t mask = 0;
+  auto produce = [&]() {
+    if (t != 0) return;
+    while (p_live && ppos < done + (uint32_t)kSlots) {
+      const bool is_out = kLayers[pc.l].is_out != 0;
+      const unsigned char* src = images + chunk_image_offset(pc.l, pc.k, kz, kParts) + (is_out ? 0 : (size_t)(2 * wg + pc.j) * kSlotBytes);
+      const uint32_t bytes = is_out ? (uint32_t)(kOutImgBytes * kParts) : (uint32_t)kSlotBytes;
+      const int s = (int)(ppos % kSlots);
+      mbar_arrive_expect_tx(full_bar(s), bytes);
+      bulk_g2s(ring + (uint32_t)s * kSlotBytes, src, bytes, full_bar(s), policy);
+      ++ppos;
+      ++pc.j;
+      p_live = pc.normalize(kz, mask, last_layer, wg);
+    }
+  };
+  float acc0[64], acc1[64], acco[8];
+  // wait for the next slot and issue its MMAs: A chunk at a_addr, 4 k-steps of 16 (x hi/lo images)
+  auto wait_slot = [&]() -> uint32_t {
+    const int s = (int)(cpos % kSlots);
+    mbar_wait(full_bar(s), (cpos / kSlots) & 1u, a.error_flag);
+    return ring + (uint32_t)s * kSlotBytes;
+  };
+  // all but the newest commit group have completed: their slots are refilled
+  auto release1 = [&]() {
+    gmma::wait<1>();
+    done = cpos - 1;
+    produce();
+  };
+  auto mma_pair = [&](uint32_t a_addr, bool fresh) {          // both quarters of the warpgroup: 2 slots, 2 commit groups
+    const uint64_t ad = gmma::desc_sw128(a_addr);
+    {
+      const uint32_t b = wait_slot();
+      gmma::fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int part = 0; part < kParts; ++part)
+          gmma::mma_f16_n128(acc0, ad + 2 * k, gmma::desc_sw128(b + part * kBSlotBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
+      gmma::commit();
+      ++cpos;
+    }
+    release1();                  // a 2-slot ring (split mode) only holds the second quarter's images once the first slot before it is free
+    {
+      const uint32_t b = wait_slot();
+      gmma::fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int part = 0; part < kParts; ++part)
+          gmma::mma_f16_n128(acc1, ad + 2 * k, gmma::desc_sw128(b + part * kBSlotBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
+      gmma::commit();
+      ++cpos;
+    }
+  };
+  auto mma_out = [&](uint32_t a_addr, bool fresh) {
+    const uint64_t ad = gmma::desc_sw128(a_addr);
+    const uint32_t b = wait_slot();
+    gmma::fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int part = 0; part < kParts; ++part)
+        gmma::mma_f16_n16(acco, ad + 2 * k, gmma::desc_sw128(b + part * kOutImgBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
+    gmma::commit();
+    ++cpos;
+  };
+  auto retire1 = release1;
+  // every commit group has completed: the accumulators may be read
+  auto retire0 = [&]() {
+    gmma::wait<0>();
+    gmma::fence_regs(acc0); gmma::fence_regs(acc1); gmma::fence_regs(acco);
+    done = cpos;
+    produce();
+  };
+  auto sync_all = [&]() { named_bar_sync(1, kThreads); };
+
+  const short2* sph_cur = sph_smem;
+  const int erow0 = 16 * w + (lane >> 2);                // accumulator rows of this thread: erow0, erow0 + 8
+  const int ecol = 2 * (lane & 3);                       // + 8 c8 (+ 128 j + 256 wg)
+
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
+    const int row0 = tile * kPts;
+    // ---------------- front-end: geometry of the tile's points ---------------------------------------------------
+    if (tid == 0) mask_smem[0] = 0ull;
+    sync_all();
+    {
+      uint32_t my_scales = 0;
+      if (tid < kPts) {
+        const int gi = row0 + tid;
+        int sx = kSphereInvalid, sy = kSphereInvalid;
+        if (gi < a.n) {
+          point_to_sphere(p, a.pts[(size_t)gi * 3 + 0], a.pts[(size_t)gi * 3 + 1], a.pts[(size_t)gi * 3 + 2], sx, sy);
+          if (a.dbg_sphere) { a.dbg_sphere[(size_t)gi * 2 + 0] = sx; a.dbg_sphere[(size_t)gi * 2 + 1] = sy; }
         }
-        // pair + tensor map: the leader arms its barrier for the bytes of BOTH CTAs; each CTA loads its own half
-        __device__ __forceinline__ void load_t(const CUtensorMap* tm, int row, uint32_t bytes) {
-          mbar_wait(bempty(rb.slot), rb.phase ^ 1, err);
-          if (crank == 0) mbar_arrive_expect_tx(bfull(rb.slot), 2 * bytes);
-          tma_load_2d_pair(smem_base + kSmemB + rb.slot * kBSlotBytes, tm, 0, row, map_to_cta(bfull(rb.slot), 0), policy);
-          rb.advance<kBSlots>();
-        }
-        // image (quarter q, part) of a chunk sits at index q * kParts + part (hi then lo in split mode)
-        __device__ __forceinline__ void quarter_t(int row0, int q) {
-          for (int part = 0; part < kParts; ++part) load_t(tmm, row0 + (q * kParts + part) * kBRows, kBSlotBytes);
-        }
-        __device__ __forceinline__ void quarter(const unsigned char* base, int q) {
-          for (int part = 0; part < kParts; ++part) load(base + (size_t)(q * kParts + part) * kBSlotBytes, kBSlotBytes);
-        }
-        __device__ __forceinline__ void op(int kind, int l, int k, int h, int) {
-          // first row of chunk k of layer l (chunk_image_offset / 128)
-          const int row0 = (int)layer_row[l] + k * (kind == OP_OUT ? kOutImgBytes / 128 : kQuarters * kBSlotBytes / 128) * kParts;
-          if (CG == 2 && use_tmap) {
-            if (kind == OP_OUT) {
-              for (int part = 0; part < kParts; ++part) load_t(tmo, (k * kParts + part) * kOutN + (int)crank * (kOutN / 2), kOutImgBytes / 2);
-              return;
-            }
-            if (kind == OP_KOUTER) { for (int i = 0; i < kHalves; ++i) quarter_t(row0, i * 2 + (int)crank); }
-            else quarter_t(row0, 2 * h + (int)crank);
-            return;
-          }
-          const unsigned char* base = images + (size_t)row0 * 128;
-          if (kind == OP_OUT) {
-            for (int part = 0; part < kParts; ++part) load(base + (size_t)part * kOutImgBytes + (size_t)crank * (kOutImgBytes / CG), kOutImgBytes / CG);
-            return;
-          }
-          if (kind == OP_KOUTER) {
-            for (int i = 0; i < kHalves; ++i) quarter(base, i * CG + (int)crank);
-          } else {
-            if (CG == 2) quarter(base, 2 * h + (int)crank);
-            else { quarter(base, 2 * h); quarter(base, 2 * h + 1); }
-          }
-        }
-        __device__ __forceinline__ void ev(int) {}
-      } prod{images, smem_base, bar0, kz, crank, a.error_flag, Ring(), l2_policy_evict_last(), &tm_main, &tm_out, a.use_tmap != 0,
-             reinterpret_cast<const volatile uint32_t*>(smem + kSmemLayerRow)};
-      uint32_t meta_phase = 0;
-      for (int grp_i = cgroup_id, it = 0; grp_i < n_groups; grp_i += n_cgroups, ++it) {
-        uint64_t mask = PRE ? 0ull : ~0ull;                    // pre-projected latents: no lin_z chunk is executed
+        // 16-bit storage: anything beyond +-32767 can only address zero padding (sphere grids are <= 16384 wide)
+        sph_smem[tid] = make_short2((short)max(min(sx, 32767), -32768), (short)max(min(sy, 32767), -32768));
         if (a.skip_zero) {
-          mbar_wait(meta_full, meta_phase, a.error_flag);        // this tile group's chunk mask is published
-          meta_phase ^= 1;
-          mask = mask_smem[it & 1];
+#pragma unroll
+          for (int s = 0; s < kScales; ++s) my_scales |= scale_taps(p, s, sx, sy).any ? (1u << s) : 0u;
         }
-        walk_tile(kz, mask, last_layer, prod);
+      }
+      if (a.skip_zero && tid < ((kPts + 31) & ~31)) {
+        const uint32_t wbits = __reduce_or_sync(0xffffffffu, my_scales);
+        if (lane == 0) {
+          const unsigned long long bits = chunk_mask_for_scales(p, wbits, kz);
+          if (bits) atomicOr((unsigned long long*)mask_smem, bits);
+        }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===================================== MMA issuer (leader CTA) ===========================================
-      struct Issuer {
-        uint32_t smem_base, bar0, tmem_base; int* err; Ring rb; int fa; uint32_t full_par;
-        uint32_t idesc_main, idesc_out; long long wa, wb; bool prof_on;
-        __device__ __forceinline__ uint32_t afull(int s) const { return bar0 + 8u * s; }
-        __device__ __forceinline__ uint32_t aempty(int s) const { return bar0 + 8u * (kASlots + s); }
-        __device__ __forceinline__ uint32_t bfull(int s) const { return bar0 + 8u * (2 * kASlots + s); }
-        __device__ __forceinline__ uint32_t bempty(int s) const { return bar0 + 8u * (2 * kASlots + kBSlots + s); }
-        __device__ __forceinline__ uint32_t hfull(int h) const { return bar0 + 8u * (2 * kASlots + 2 * kBSlots + h); }
-        __device__ __forceinline__ void wait_a(int slot) {
-          const long long t0 = (PROF && prof_on) ? clock64() : 0;
-          mbar_wait_cluster(afull(slot), (full_par >> slot) & 1u, err);
-          if (PROF && prof_on) wa += clock64() - t0;
-          full_par ^= 1u << slot;
-        }
-        // weight image(s) of one accumulator column group: wait, 4 MMAs per image pair, release
-        __device__ __forceinline__ void mma_group(uint64_t adesc, int n_img, uint32_t dcol, uint32_t idesc, bool fresh) {
-          if constexpr (SPLIT) {
-            // hi image then lo image of every column group, slot by slot (the ring is consumed in order)
-            for (int i = 0; i < n_img; ++i)
-              for (int part = 0; part < 2; ++part) {
-                const long long t0 = (PROF && prof_on) ? clock64() : 0;
-                mbar_wait_cluster(bfull(rb.slot), rb.phase, err);
-                if (PROF && prof_on) wb += clock64() - t0;
-                const int slot = rb.slot;
-                rb.advance<kBSlots>();
-                tc_fence_after();
-                const uint64_t bdesc = make_desc_sw128(smem_base + kSmemB + slot * kBSlotBytes);
-#pragma unroll
-                for (int k = 0; k < kChunkK / 16; ++k)
-                  umma_f16<CG>(tmem_base + dcol + (uint32_t)(i * kMmaN), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                               (fresh && k == 0 && part == 0) ? 0u : 1u);
-                umma_commit<CG>(bempty(slot));
-              }
-            return;
-          }
-          int bs[2];
-          for (int i = 0; i < n_img; ++i) {
-            const long long t0 = (PROF && prof_on) ? clock64() : 0;
-            mbar_wait_cluster(bfull(rb.slot), rb.phase, err);
-            if (PROF && prof_on) wb += clock64() - t0;
-            bs[i] = rb.slot;
-            rb.advance<kBSlots>();
-          }
-          tc_fence_after();
-          for (int i = 0; i < n_img; ++i) {
-            const uint64_t bdesc = make_desc_sw128(smem_base + kSmemB + bs[i] * kBSlotBytes);
-#pragma unroll
-            for (int k = 0; k < kChunkK / 16; ++k)     // +32 bytes per UMMA_K=16 fp16 inside the swizzle row: start address += 2
-              umma_f16<CG>(tmem_base + dcol + (uint32_t)(i * kMmaN), adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                           (fresh && k == 0) ? 0u : 1u);
-          }
-          for (int i = 0; i < n_img; ++i) umma_commit<CG>(bempty(bs[i]));
-        }
-        __device__ __forceinline__ void op(int kind, int l, int k, int h, int fresh) {
-          if (kind == OP_KOUTER) {
-            const int slot = fa;
-            fa = (fa + 1) & 3;
-            wait_a(slot);
-            tc_fence_after();
-            const uint64_t adesc = make_desc_sw128(smem_base + kSmemA + slot * kASlotBytes);
-            // CG=2: 2 images = 2 halves of 256 columns; CG=1: 4 images = 4 quarters of 128 columns
-            mma_group(adesc, 2, 0u, idesc_main, fresh != 0);
-            if (CG == 1) mma_group(adesc, 2, 2u * kMmaN, idesc_main, fresh != 0);
-            umma_commit<CG>(aempty(slot));
-          } else if (kind == OP_SGROUP) {
-            const uint64_t adesc = make_desc_sw128(smem_base + kSmemA + k * kASlotBytes);
-            mma_group(adesc, CG == 2 ? 1 : 2, (uint32_t)(h * 256), idesc_main, fresh != 0);
-          } else {
-            wait_a(k);
-            tc_fence_after();
-            const uint64_t adesc = make_desc_sw128(smem_base + kSmemA + k * kASlotBytes);
-            mma_group(adesc, 1, 0u, idesc_out, fresh != 0);
-            umma_commit<CG>(aempty(k));
-          }
-        }
-        __device__ __forceinline__ void ev(int e) {
-          switch (e) {
-            case EV_PRE_S1: for (int s = 0; s < 4; ++s) wait_a(s); tc_fence_after(); break;     // A chunks 0-3 ready, half 0 drained
-            case EV_PRE_S2: for (int s = 4; s < 8; ++s) wait_a(s); tc_fence_after(); break;     // A chunks 4-7 ready, half 1 drained
-            case EV_BANK0_FREE: for (int s = 0; s < 4; ++s) umma_commit<CG>(aempty(s)); break;
-            case EV_HALF0: umma_commit<CG>(hfull(0)); break;
-            case EV_BANK1_FREE_HALF1: for (int s = 4; s < 8; ++s) umma_commit<CG>(aempty(s)); umma_commit<CG>(hfull(1)); break;
-            case EV_ALL: umma_commit<CG>(hfull(0)); umma_commit<CG>(hfull(1)); break;
-            case EV_OUT: umma_commit<CG>(hfull(0)); break;
-          }
-        }
-      } iss{smem_base, bar0, tmem_base, a.error_flag, Ring(), 0, 0u,
-            make_idesc(kTileM * CG, kMmaN), make_idesc(kTileM * CG, kOutN), 0, 0, PROF && a.prof != nullptr};
-      uint32_t meta_phase = 0;
-      for (int grp_i = cgroup_id, it = 0; grp_i < n_groups; grp_i += n_cgroups, ++it) {
-        uint64_t mask = PRE ? 0ull : ~0ull;
-        if (a.skip_zero) {
-          mbar_wait(meta_full, meta_phase, a.error_flag);
-          meta_phase ^= 1;
-          mask = mask_smem[it & 1];
-        }
-        iss.fa = 0;
-        walk_tile(kz, mask, last_layer, iss);
-      }
-      if (PROF && iss.prof_on) { a.prof[(size_t)blockIdx.x * 16 + 8] = (unsigned long long)iss.wa; a.prof[(size_t)blockIdx.x * 16 + 9] = (unsigned long long)iss.wb; }
-    } else if (CG == 2 && lane == 0 && !leader && !a.use_tmap) {
-      // ===================================== weight-full relay (peer CTA; only without tensor-map loads) =========
-      // walks the same image sequence as the producer; when a local image has landed, arrives on the leader's
-      // barrier of the same slot (the leader's MMA reads this CTA's half of B through the pair datapath)
-      struct Relay {
-        uint32_t bar0; int* err; Ring rb;
-        __device__ __forceinline__ void fwd() {
-          const uint32_t bar = bar0 + 8u * (2 * kASlots + rb.slot);
-          mbar_wait(bar, rb.phase, err);
-          mbar_arrive_remote(map_to_cta(bar, 0));
-          rb.advance<kBSlots>();
-        }
-        __device__ __forceinline__ void op(int kind, int, int, int, int) {
-          const int n = (kind == OP_KOUTER ? kHalves : 1) * kParts;
-          for (int i = 0; i < n; ++i) fwd();
-        }
-        __device__ __forceinline__ void ev(int) {}
-      } rel{bar0, a.error_flag, Ring()};
-      uint32_t meta_phase = 0;
-      for (int grp_i = cgroup_id, it = 0; grp_i < n_groups; grp_i += n_cgroups, ++it) {
-        uint64_t mask = PRE ? 0ull : ~0ull;
-        if (a.skip_zero) {
-          mbar_wait(meta_full, meta_phase, a.error_flag);
-          meta_phase ^= 1;
-          mask = mask_smem[it & 1];
-        }
-        walk_tile(kz, mask, last_layer, rel);
-      }
-    }
-  } else {
-    // ===================================== workers =============================================================
-    const int wt = threadIdx.x - 64;             // 0..255
-    const int q4 = warp & 3;                     // TMEM lane quarter this warp may access
-    const int sub = (warp >= 6) ? 1 : 0;         // warps (2,6),(3,7),(4,8),(5,9) share a quarter: 128 columns each per half
-    const int erow = q4 * 32 + lane;             // epilogue row
-    const float* bias = reinterpret_cast<const float*>(a.wblob);
-    float4* scratch4 = reinterpret_cast<float4*>(a.scratch + (size_t)blockIdx.x * kTileM * kHidden);
-    int fa = 0;                                  // FIFO position in A bank 0 (slots 0..3): x / latent chunks
-    uint32_t fill_par = 0;                       // per-slot parity of the number of fills done by the workers
-    uint32_t half_par = 0;                                       // bit p: parity of accumulator half p's "full" barrier
-    uint32_t meta_phase = 0;
-    uint32_t zpar = 0;                           // parity per zbar slot
-    unsigned char* zc_base = a.zcache ? a.zcache + (size_t)blockIdx.x * kZCache * kASlotBytes : nullptr;
-    const uint64_t zpolicy = l2_policy_evict_last();
+    sync_all();
+    mask = PRE ? 0ull : (a.skip_zero ? mask_smem[0] : ~0ull);
+    // weight stream of this tile: prime the ring (every slot of the previous tile has completed)
+    pc = Cursor();
+    p_live = pc.normalize(kz, mask, last_layer, wg);
+    produce();
 
-    // -- helpers -------------------------------------------------------------------------------------------
-    auto wait_slot_free = [&](int slot) { mbar_wait(a_empty(slot), ((fill_par >> slot) & 1u) ^ 1u, a.error_flag); };
-    // A-full barriers live in the leader CTA: the MMA issuer there consumes the A tiles of both CTAs of a pair
-    auto arrive_a_full = [&](int slot) {
-      if constexpr (CG == 1) mbar_arrive(a_full(slot));
-      else mbar_arrive_remote(map_to_cta(a_full(slot), 0));
-    };
-    auto publish_slot = [&](int slot) {          // all of this warp's writes to the A slot are done
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) arrive_a_full(slot);
-      fill_par ^= 1u << slot;
-    };
-    // cycle accounting (one thread per CTA: first worker lane): 0 front-end, 1 gather passes, 2 waiting for ACC,
-    // 3 epilogue E1 halves, 4 whole kernel, 5 E2 halves, 6 E3 halves, 7 blocked on A slots during gather
-    const bool prof_on = PROF && (a.prof != nullptr) && (wt == 0);
-    long long pc[PROF ? 8 : 1] = {0};
-    long long pt = prof_on ? clock64() : 0;
-    const long long pt_start = pt;
-    auto lap = [&](int idx) {
-      if constexpr (PROF) { if (prof_on) { const long long t = clock64(); pc[idx] += t - pt; pt = t; } }
-    };
-
-    for (int grp_i = cgroup_id, it = 0; grp_i < n_groups; grp_i += n_cgroups, ++it) {
-      const int tile = grp_i * CG + (int)crank;
-      const int row0 = tile * kPts;
-      fa = 0;
-      // ---------------- front-end: geometry of a tile's 128 points (threads 0..127, one point each) -----------
-      // With zero-chunk skipping in a CTA pair, threads 128..255 (idle here otherwise) run the same geometry for the
-      // PEER's tile, so that both CTAs derive the identical union chunk mask locally (no cross-CTA exchange).
-      // The geometry of tile it+1 is computed while tile `it` waits for its last fc_1 (double-buffered sph / mask).
-      auto geometry = [&](int grp, int it_) {
-        uint32_t my_scales = 0;
-        const bool own = wt < kPts;
-        const bool for_peer = wt >= kTileM && wt < kTileM + kPts;
-        const int trow = own ? wt : wt - kTileM;
-        const int ttile = grp * CG + (own ? (int)crank : (1 - (int)crank));
-        if (own || (for_peer && CG == 2 && a.skip_zero)) {
-          const int gi = ttile * kPts + trow;
-          int sx = kSphereInvalid, sy = kSphereInvalid;
-          if (gi < a.n) {
-            point_to_sphere(p, a.pts[(size_t)gi * 3 + 0], a.pts[(size_t)gi * 3 + 1], a.pts[(size_t)gi * 3 + 2], sx, sy);
-            if (own && a.dbg_sphere) { a.dbg_sphere[(size_t)gi * 2 + 0] = sx; a.dbg_sphere[(size_t)gi * 2 + 1] = sy; }
-          }
-          // 16-bit storage: anything beyond +-32767 can only address zero padding (sphere grids are <= 16384 wide)
-          if (own) sph_smem[(it_ & 1) * kTileM + wt] = make_short2((short)max(min(sx, 32767), -32768), (short)max(min(sy, 32767), -32768));
-          if (a.skip_zero) {
+    // pre-projected latents: table rows of the two points whose accumulator rows this thread finishes
+    const unsigned char* pre_row[2] = {nullptr, nullptr};
+    if constexpr (PRE) {
 #pragma unroll
-            for (int s = 0; s < kScales; ++s) my_scales |= scale_taps(p, s, sx, sy).any ? (1u << s) : 0u;
-          }
-        }
-        if (a.skip_zero) {
-          // chunk mask of that tile group: its buffer was zeroed at the top of the previous tile
-          const uint32_t wbits = __reduce_or_sync(0xffffffffu, my_scales);
-          if (lane == 0) {
-            const unsigned long long bits = chunk_mask_for_scales(p, wbits, kz);
-            if (bits) atomicOr((unsigned long long*)&mask_smem[it_ & 1], bits);
-            mbar_arrive(meta_full);
-          }
-        }
-      };
-      if (it == 0 || a.debug_layer >= 0) geometry(grp_i, it);
-      const short2* sph_cur = sph_smem + (it & 1) * kTileM;
-      uint64_t mask = PRE ? 0ull : ~0ull;
-      if (a.skip_zero) {
-        if (wt == 0) mask_smem[(it + 1) & 1] = 0ull;          // buffer of the NEXT tile group (filled later in this tile)
-        mbar_wait(meta_full, meta_phase, a.error_flag);
-        meta_phase ^= 1;
-        mask = mask_smem[it & 1];
-      }
-      named_bar_sync(1, kWorkerThreads);          // sph_smem visible to all workers
-      // pre-projected latents: table row of the point this lane finishes in the epilogues (zero row outside the grid)
-      const unsigned char* pre_row = nullptr;
-      if constexpr (PRE) {
-        const short2 sp = sph_cur[SPLIT ? ((q4 & 1) * 32 + lane) : erow];
+      for (int hh = 0; hh < 2; ++hh) {
+        const short2 sp = sph_cur[(erow0 + 8 * hh) % kPts];
         const bool in = sp.x >= 0 && sp.x < a.pre_W1 && sp.y >= 0 && sp.y < a.pre_H1;
         const size_t ridx = in ? (size_t)sp.y * a.pre_W1 + sp.x : (size_t)a.pre_W1 * a.pre_H1;
-        pre_row = a.preproj + ridx * (size_t)(SRF_NUM_BLOCKS * kHidden * (SPLIT ? 4 : 2));
+        pre_row[hh] = a.preproj + ridx * (size_t)(SRF_NUM_BLOCKS * kHidden * (SPLIT ? 4 : 2));
       }
+    }
 
-      // ---------------- L0: x chunk = [pe(39) | viewdir(3) | 0] as fp16 (FIFO slot) ---------------------------
-      {
-        const int slot = fa;
-        fa = (fa + 1) & 3;
-        wait_slot_free(slot);
-        {
-          // two threads per row: thread wt < 128 writes granules 0-2 (x,y,z + the first 21 encodings), thread
-          // wt-128 writes granules 3-7 (the other 15 encodings, the view direction, zero padding) and issues the
-          // L2 prefetches of the row's gather taps
-          const bool first = wt < kTileM;
-          const int xrow = first ? wt : wt - kTileM;
-          const bool xlive = xrow < kPts;           // split mode: rows 64..127 are the low parts, written by the thread of row-64
-          const int gi = xlive ? row0 + xrow : a.n;
-          const uint32_t slot_addr = smem_base + kSmemA + slot * kASlotBytes;
-          float qx = 0.f, qy = 0.f, qz = 0.f;
-          if (gi < a.n) { qx = a.pts[(size_t)gi * 3 + 0]; qy = a.pts[(size_t)gi * 3 + 1]; qz = a.pts[(size_t)gi * 3 + 2]; }
-          const float kPi = 3.14159274101257324f, kHalfPi = 1.57079637050628662f;
-          auto sel3 = [](int i, float v0, float v1, float v2) { return i == 0 ? v0 : (i == 1 ? v1 : v2); };   // no indexed register arrays
-          // value of x_in index idx (0..63) for this row: pe.py:32-43 order, then viewdir, then zeros.  idx is a RUN-TIME value
-          // (uniform per warp): the granules are produced by a rolled loop, so the kernel holds 8 copies of sinf (one per value of
-          // a granule, for ILP) instead of 36 -- each copy drags its never-taken large-argument path (~110 instructions) along.
-          auto xval = [&](int idx, const float* vd) -> float {
-            if (gi >= a.n) return 0.0f;
-            if (idx < 3) return sel3(idx, qx, qy, qz);
-            if (idx < 3 + 36) {
-              const int j = idx - 3, fp = j / 3, cc = j - 3 * fp;    // fp = 2*k + phase
-              float arg = fmul(sel3(cc, qx, qy, qz), kPi * (float)(1 << (fp >> 1)));    // pi * 2^k: exact scaling of the fp32 constant
-              if (fp & 1) arg = fadd(kHalfPi, arg);
-              return sinf(arg);
-            }
-            if (idx < kDX) return sel3(idx - 39, vd[0], vd[1], vd[2]);
-            return 0.0f;
-          };
-          // one 16-byte granule (8 values) of row xrow; split mode: high parts to xrow, low parts to xrow + 64
-          auto put_granule = [&](int g, const float* vd) {
-            float v[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = xval(8 * g + j, vd);
-            if constexpr (SPLIT) {
-              uint32_t hi[4], lo[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) split_half2(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
-              sts128(slot_addr + sw128_offset(xrow, g), hi[0], hi[1], hi[2], hi[3]);
-              sts128(slot_addr + sw128_offset(xrow + kPts, g), lo[0], lo[1], lo[2], lo[3]);
-            } else {
-              sts128(slot_addr + sw128_offset(xrow, g), pack_half2(v[0], v[1]), pack_half2(v[2], v[3]), pack_half2(v[4], v[5]),
-                     pack_half2(v[6], v[7]));
-            }
-          };
-          float vd[3] = {0.f, 0.f, 0.f};
-          if (xlive && !first && gi < a.n) {
-            const float* vp = a.viewdir + (size_t)(gi / a.n_per) * 3;
-            vd[0] = vp[0]; vd[1] = vp[1]; vd[2] = vp[2];
-          }
-          if (xlive) {
-            // (a row of the tile with !xlive belongs to the thread of point row - 64)
-            const int g_end = first ? 3 : 8;
-#pragma unroll 1
-            for (int g = first ? 0 : 3; g < g_end; ++g) put_granule(g, vd);
-          }
-          if (xlive && !first) {
-            // warm L2 with the taps this row will gather from the (usually in-bounds) fine scales: the gather runs
-            // thousands of cycles later and then sees L2 instead of HBM latency
-            const short2 sp16 = sph_cur[xrow];
-            const int2 sp = make_int2(sp16.x, sp16.y);
-            const int esz = p.feat_fp16 ? 2 : 4;
-            if constexpr (PRE) {
-              // warm L2 with this point's table row (3 x 512 values): the E1 epilogues read it thousands of cycles later
-              if (sp.x >= 0 && sp.x < a.pre_W1 && sp.y >= 0 && sp.y < a.pre_H1) {
-                constexpr int kRowBytes = SRF_NUM_BLOCKS * kHidden * (SPLIT ? 4 : 2);
-                const unsigned char* rowp = a.preproj + ((size_t)sp.y * a.pre_W1 + sp.x) * kRowBytes;
-                for (int b = 0; b < kRowBytes; b += 128) prefetch_l2(rowp + b);
-              }
-            } else
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-              const Taps tp = scale_taps(p, s, sp.x, sp.y);
-              if (tp.any) {
-                const int bytes = p.C[s] * esz;
-#pragma unroll
-                for (int t = 0; t < 4; ++t)
-                  if (tp.off[t] >= 0) {
-                    const char* base = reinterpret_cast<const char*>(p.feat[s]) + (size_t)tp.off[t] * esz;
-                    for (int b = 0; b < bytes; b += 128) prefetch_l2(base + b);
-                    prefetch_l2(base + bytes - 4);
-                  }
-              }
-            }
-          }
+    // ---------------- x chunk = [pe(39) | viewdir(3) | 0] as fp16 ----------------------------------------------------
+    if (tid < 2 * kPts) {
+      // two threads per point: thread tid < kPts writes granules 0-2 (x,y,z + the first 21 encodings), the other
+      // granules 3-7 (the other 15 encodings, the view direction, zero padding)
+      const bool first = tid < kPts;
+      const int xrow = first ? tid : tid - kPts;
+      const int gi = row0 + xrow;
+      const uint32_t slot_addr = smem_base + kSmemX;
+      float qx = 0.f, qy = 0.f, qz = 0.f;
+      if (gi < a.n) { qx = a.pts[(size_t)gi * 3 + 0]; qy = a.pts[(size_t)gi * 3 + 1]; qz = a.pts[(size_t)gi * 3 + 2]; }
+      const float kPi = 3.14159274101257324f, kHalfPi = 1.57079637050628662f;
+      auto sel3 = [](int i, float v0, float v1, float v2) { return i == 0 ? v0 : (i == 1 ? v1 : v2); };   // no indexed register arrays
+      // value of x_in index idx (0..63) for this row: pe.py:32-43 order, then viewdir, then zeros.  idx is a run-time value
+      // (the granules are produced by a rolled loop, so the kernel holds 8 copies of sinf instead of 36)
+      auto xval = [&](int idx, const float* vd) -> float {
+        if (gi >= a.n) return 0.0f;
+        if (idx < 3) return sel3(idx, qx, qy, qz);
+        if (idx < 3 + 36) {
+          const int j = idx - 3, fp = j / 3, cc = j - 3 * fp;    // fp = 2*k + phase
+          float arg = fmul(sel3(cc, qx, qy, qz), kPi * (float)(1 << (fp >> 1)));    // pi * 2^k: exact scaling of the fp32 constant
+          if (fp & 1) arg = fadd(kHalfPi, arg);
+          return sinf(arg);
         }
-        publish_slot(slot);
+        if (idx < kDX) return sel3(idx - 39, vd[0], vd[1], vd[2]);
+        return 0.0f;
+      };
+      float vd[3] = {0.f, 0.f, 0.f};
+      if (!first && gi < a.n) {
+        const float* vp = a.viewdir + (size_t)(gi / a.n_per) * 3;
+        vd[0] = vp[0]; vd[1] = vp[1]; vd[2] = vp[2];
       }
-
-      // ---------------- gather pass: produces the latent chunks of one lin_z layer through the bank-0 FIFO ------
-      // thread -> 4 items per chunk: rows (wt/8) + 32*i, granule (8 channels = 16 B of fp16) g = wt % 8.
-      // Per row only (element offset of the north-west tap, x/y fractional weights, 4 validity bits) is kept in
-      // registers; the 4 tap weights are re-derived (same products as scale_taps) when a chunk is gathered.
-      // The gathered chunks of the fine scales (chunks 0..kZCache-1: the ones that normally carry data) are identical
-      // for lin_z0/1/2: pass 0 also writes their fp16 tile images to an L2-resident per-CTA cache, passes 1 and 2
-      // bring them back with one cp.async.bulk each (all in flight together) instead of gathering again.
-      constexpr int kItems = kPts / 32;           // rows per thread and chunk: (wt/8) + 32*i
-      auto gather_pass = [&](int pass) {
-        const int g = wt & 7;
-        int first_c = 0;
-        if (pass > 0 && zc_base) {
-          named_bar_sync(1, kWorkerThreads);      // pass-0 cache stores (+ their proxy fences) of every worker are done
-          int zs[kZCache];
-          int nz = 0;
-          for (int c = 0; c < kZCache && c < kz; ++c) {
-            if (!((mask >> c) & 1ull)) continue;
-            const int slot = fa;
-            fa = (fa + 1) & 3;
-            wait_slot_free(slot);
-            if (wt == 0) {
-              mbar_arrive_expect_tx(zbar(slot), kASlotBytes);
-              bulk_g2s(smem_base + kSmemA + slot * kASlotBytes, zc_base + (size_t)c * kASlotBytes, kASlotBytes, zbar(slot), zpolicy);
-            }
-            zs[nz++] = slot;
-          }
-          for (int i = 0; i < nz; ++i) {
-            mbar_wait(zbar(zs[i]), (zpar >> zs[i]) & 1u, a.error_flag);
-            zpar ^= 1u << zs[i];
-            publish_slot(zs[i]);
-          }
-          first_c = kZCache;
-        }
-        int cur_scale = -1;
-        int t_off[4];              // offset of tap 0 (may be "virtual" when tap 0 itself is out of range)
-        uint32_t t_ok[4];          // bit t = tap t in range
-        float t_w[4], t_n[4];      // fractional x / y weights (w, n of scale_taps)
-        int dxo = 0, dyo = 0;      // element strides to the east / south tap
-        for (int c = first_c; c < kz; ++c) {
-          if (!((mask >> c) & 1ull)) continue;
-          const int ch = c * kChunkK + g * 8;                     // first of this thread's 8 channels
-          // pass 0: mirror the tile image of the cached chunks to global (same swizzled byte order as the slot)
-          unsigned char* zc = (pass == 0 && zc_base && c < kZCache) ? zc_base + (size_t)c * kASlotBytes : nullptr;
-          auto emit = [&](int row, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t slot_addr_) {
-            const uint32_t off = sw128_offset(row, g);
-            sts128(slot_addr_ + off, w0, w1, w2, w3);
-            if (zc) *reinterpret_cast<uint4*>(zc + off) = make_uint4(w0, w1, w2, w3);
-          };
-          // 8 gathered channels of one point: fp16 operands (split mode: high parts to `row`, low parts to row + 64)
-          auto emit_vals = [&](int row, const float (&v)[8], uint32_t slot_addr_) {
-            if constexpr (SPLIT) {
-              uint32_t hi[4], lo[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) split_half2(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
-              emit(row, hi[0], hi[1], hi[2], hi[3], slot_addr_);
-              emit(row + kPts, lo[0], lo[1], lo[2], lo[3], slot_addr_);
-            } else {
-              emit(row, pack_half2(v[0], v[1]), pack_half2(v[2], v[3]), pack_half2(v[4], v[5]), pack_half2(v[6], v[7]), slot_addr_);
-            }
-          };
-          auto emit_zero = [&](int row, uint32_t slot_addr_) {
-            emit(row, 0u, 0u, 0u, 0u, slot_addr_);
-            if constexpr (SPLIT) emit(row + kPts, 0u, 0u, 0u, 0u, slot_addr_);
-          };
-          int s = -1;
-#pragma unroll
-          for (int i = 0; i < kScales; ++i)
-            if (ch >= p.ch_off[i] && ch < p.ch_off[i + 1]) s = i;
-          if (s >= 0 && s != cur_scale) {
-            dxo = p.C[s]; dyo = p.W[s] * p.C[s];
-#pragma unroll
-            for (int i = 0; i < kItems; ++i) {
-              const short2 sp16 = sph_cur[(wt >> 3) + 32 * i];
-              const int2 sp = make_int2(sp16.x, sp16.y);
-              const Taps tp = scale_taps(p, s, sp.x, sp.y);
-              t_ok[i] = (tp.off[0] >= 0 ? 1u : 0u) | (tp.off[1] >= 0 ? 2u : 0u) | (tp.off[2] >= 0 ? 4u : 0u) | (tp.off[3] >= 0 ? 8u : 0u);
-              // off[t] = off0 + (t&1)*dxo + (t>>1)*dyo for in-range taps -> recover off0 from any valid tap
-              int o0 = 0;
-              if (tp.off[0] >= 0) o0 = tp.off[0];
-              else if (tp.off[1] >= 0) o0 = tp.off[1] - dxo;
-              else if (tp.off[2] >= 0) o0 = tp.off[2] - dyo;
-              else if (tp.off[3] >= 0) o0 = tp.off[3] - dxo - dyo;
-              t_off[i] = o0;
-              t_w[i] = tp.fx; t_n[i] = tp.fy;
-            }
-            cur_scale = s;
-          }
-          const int slot = fa;
-          fa = (fa + 1) & 3;
-          if constexpr (PROF) {
-            const long long tw = prof_on ? clock64() : 0;
-            wait_slot_free(slot);
-            if (prof_on) pc[7] += clock64() - tw;
-          } else {
-            wait_slot_free(slot);
-          }
-          const uint32_t slot_addr = smem_base + kSmemA + slot * kASlotBytes;
-          // element index of this thread's first channel inside the scale's HWC map (features are float or half)
-          const char* fbytes = (s >= 0) ? reinterpret_cast<const char*>(p.feat[s]) : nullptr;
-          const int ch_in = (s >= 0) ? ch - p.ch_off[s] : 0;
-          const bool f16 = p.feat_fp16 != 0;
-          uint32_t any_live = 0u;
-          if (s >= 0) {
-#pragma unroll
-            for (int u = 0; u < kItems; ++u) any_live |= t_ok[u];
-          }
-          if (!any_live) {
-            // nothing to gather for this thread's rows (the normal case for the coarse scales): zeros
-#pragma unroll
-            for (int u = 0; u < kItems; ++u) emit_zero((wt >> 3) + 32 * u, slot_addr);
-          } else if (f16) {
-            // fp16 pyramid: a tap of 8 channels is ONE 128-bit load -> all 16 taps of the thread's 4 items are
-            // requested together (one memory round trip per chunk)
-            uint4 raw[kItems][4];
-#pragma unroll
-            for (int u = 0; u < kItems; ++u) {
-              const uint32_t ok = (s >= 0) ? t_ok[u] : 0u;
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                if ((ok >> t) & 1u) {
-                  const size_t eidx = (size_t)(ch_in + t_off[u] + (t & 1) * dxo + (t >> 1) * dyo);
-                  raw[u][t] = __ldg(reinterpret_cast<const uint4*>(fbytes + eidx * 2));
-                } else {
-                  raw[u][t] = make_uint4(0u, 0u, 0u, 0u);
-                }
-              }
-            }
-#pragma unroll
-            for (int u = 0; u < kItems; ++u) {
-              const int row = (wt >> 3) + 32 * u;
-              if (!((s >= 0) && t_ok[u])) { emit_zero(row, slot_addr); continue; }
-              const float w = t_w[u], n = t_n[u];
-              const float e = fsub(1.0f, w), so = fsub(1.0f, n);
-              const float tw4[4] = {fmul(so, e), fmul(so, w), fmul(n, e), fmul(n, w)};     // nw, ne, sw, se
-              float acc[8];
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                const float wt_ = tw4[t];
-                const uint32_t rw[4] = {raw[u][t].x, raw[u][t].y, raw[u][t].z, raw[u][t].w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&rw[q]));
-                  if (t == 0) { acc[2 * q] = fmul(f.x, wt_); acc[2 * q + 1] = fmul(f.y, wt_); }
-                  else { acc[2 * q] = fadd(acc[2 * q], fmul(f.x, wt_)); acc[2 * q + 1] = fadd(acc[2 * q + 1], fmul(f.y, wt_)); }
-                }
-              }
-              emit_vals(row, acc, slot_addr);
-            }
-          } else {
-          // two items at a time: their (up to) 16 tap loads are requested before the first one is consumed
-#pragma unroll
-          for (int ib = 0; ib < kItems; ib += 2) {
-            const bool live0 = (s >= 0) && t_ok[ib], live1 = (s >= 0) && t_ok[ib + 1];
-            if (!live0 && !live1) {                               // the common case for the coarse scales
-              emit_zero((wt >> 3) + 32 * ib, slot_addr);
-              emit_zero((wt >> 3) + 32 * (ib + 1), slot_addr);
-              continue;
-            }
-            float4 v[2][4][2];
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const uint32_t ok = (s >= 0) ? t_ok[ib + u] : 0u;
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                if ((ok >> t) & 1u) {
-                  const size_t eidx = (size_t)(ch_in + t_off[ib + u] + (t & 1) * dxo + (t >> 1) * dyo);
-                  const float4* src = reinterpret_cast<const float4*>(fbytes + eidx * 4);
-                  v[u][t][0] = __ldg(src);
-                  v[u][t][1] = __ldg(src + 1);
-                } else {
-                  v[u][t][0] = make_float4(0.f, 0.f, 0.f, 0.f);
-                  v[u][t][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-              }
-            }
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int row = (wt >> 3) + 32 * (ib + u);
-              const float w = t_w[ib + u], n = t_n[ib + u];
-              const float e = fsub(1.0f, w), so = fsub(1.0f, n);
-              const float tw4[4] = {fmul(so, e), fmul(so, w), fmul(n, e), fmul(n, w)};     // nw, ne, sw, se
-              float acc[8];
-              // out = ((v_nw*nw + v_ne*ne) + v_sw*sw) + v_se*se : separate roundings like ATen's CPU kernel
-              // (an out-of-range tap contributes an exact +0)
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                const float wt_ = tw4[t];
-                const float4 a0 = v[u][t][0], a1 = v[u][t][1];
-                if (t == 0) {
-                  acc[0] = fmul(a0.x, wt_); acc[1] = fmul(a0.y, wt_); acc[2] = fmul(a0.z, wt_); acc[3] = fmul(a0.w, wt_);
-                  acc[4] = fmul(a1.x, wt_); acc[5] = fmul(a1.y, wt_); acc[6] = fmul(a1.z, wt_); acc[7] = fmul(a1.w, wt_);
-                } else {
-                  acc[0] = fadd(acc[0], fmul(a0.x, wt_)); acc[1] = fadd(acc[1], fmul(a0.y, wt_));
-                  acc[2] = fadd(acc[2], fmul(a0.z, wt_)); acc[3] = fadd(acc[3], fmul(a0.w, wt_));
-                  acc[4] = fadd(acc[4], fmul(a1.x, wt_)); acc[5] = fadd(acc[5], fmul(a1.y, wt_));
-                  acc[6] = fadd(acc[6], fmul(a1.z, wt_)); acc[7] = fadd(acc[7], fmul(a1.w, wt_));
-                }
-              }
-              emit_vals(row, acc, slot_addr);
-            }
-          }
-          }
-          publish_slot(slot);
-        }
-        // the cache writes above are generic-proxy global stores; the later cp.async.bulk reads them via the async proxy
-        if (pass == 0 && zc_base) asm volatile("fence.proxy.async.global;" ::: "memory");
-      };
-
-      // ---------------- epilogue of one accumulator half: TMEM -> [+bias (+h)] -> (scratch) -> relu -> fp16 -------
-      //   part: 0 -> columns 0..255 -> A slots 0..3 ; 1 -> columns 256..511 -> A slots 4..7.  This warp: 128 columns
-      //   (2 A chunks).  bias_idx: header vector; use_h: add the fp32 hidden state from scratch; write_h: store it.
-      //   16-column groups; TMEM load, scratch and bias of group g+1 are in flight while group g is processed.
-      // SASS of the first version of this epilogue (run-time flags, one register set copied forward): ~206 instructions per
-      // 16-column group and lane (48 FADD, 36 register MOVs from copying the prefetched operands, 32 half->float conversions,
-      // 16 packs, flag-dependent selects) for 16 elements -- with two warps per scheduler the epilogues are ISSUE-bound
-      // (2 x 206 issue slots ~ the measured 450 cycles per group), not latency-bound.  Here every flag is a compile-time
-      // constant of the call site (no selects, no +0 adds), the operands of even and odd groups live in two register sets
-      // that are consumed in place (no MOVs), and per-lane base pointers advance by constants.  The body is force-inlined:
-      // an out-of-line closure keeps every captured variable in local memory (measured: 1.4x slower epilogues).
-      auto epilogue_half_lean = [&](auto use_h_c, auto write_h_c, auto use_p_c, int part, int bias_idx) __attribute__((always_inline)) {
-        constexpr bool USE_H = decltype(use_h_c)::value, WRITE_H = decltype(write_h_c)::value, USE_P = decltype(use_p_c)::value;
-        lap(1);
-        const uint32_t trow = tmem_base + ((uint32_t)(q4 * 32) << 16);
-        const int col0 = part * 256 + sub * 128;
-        const float4* bp = reinterpret_cast<const float4*>(bias + (size_t)bias_idx * kHidden) + (col0 >> 2);        // 4 float4 per group
-        uint4* h8 = reinterpret_cast<uint4*>(scratch4) + (size_t)(col0 >> 3) * kTileM + erow;                       // fp16 h: [col/8][row], 2 per group
-        float4* h4 = scratch4 + (size_t)(col0 >> 2) * kTileM + erow;                                                // fp32 h: [col/4][row], 4 per group
-        const uint4* pp = reinterpret_cast<const uint4*>(pre_row + (size_t)bias_idx * kHidden * 2) + (col0 >> 3);   // table row: 2 uint4 per group
-        struct Set { uint32_t v[16]; uint4 h[H16 ? 2 : 4]; uint4 p[2]; };
-        Set A, B;
-        auto load_hp = [&](Set& s, int g) {                     // accumulator-independent operands of group g
-          if constexpr (USE_H) {
-            if constexpr (H16) { s.h[0] = h8[(size_t)(2 * g) * kTileM]; s.h[1] = h8[(size_t)(2 * g + 1) * kTileM]; }
-            else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) s.h[j] = *reinterpret_cast<const uint4*>(h4 + (size_t)(4 * g + j) * kTileM);
-            }
-          }
-          if constexpr (USE_P) { s.p[0] = __ldg(pp + 2 * g); s.p[1] = __ldg(pp + 2 * g + 1); }
-        };
-        load_hp(A, 0);
-        load_hp(B, 1);
-        mbar_wait(half_full(part), (half_par >> part) & 1u, a.error_flag);
-        half_par ^= 1u << part;
-        tc_fence_after();
-        lap(2);
-        tmem_ld16(trow + (uint32_t)col0, A.v);
-        auto body = [&](Set& cur, Set& nxt, int g) __attribute__((always_inline)) {
-          const int col = col0 + g * 16;
-          float4 bb[4];
-          if constexpr (!USE_P) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bb[j] = __ldg(bp + 4 * g + j);
-          }
-          tmem_ld_wait();
-          if (g < 7) tmem_ld16(trow + (uint32_t)(col + 16), nxt.v);
-          const int slot = col >> 6;
-          if ((g & 3) == 0) wait_slot_free(slot);
-          const uint32_t srow = smem_base + kSmemA + slot * kASlotBytes + (uint32_t)(erow * 128);
-#pragma unroll
-          for (int gq = 0; gq < 2; ++gq) {                      // 2 granules of 8 columns
-            float r[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) r[e] = __uint_as_float(cur.v[gq * 8 + e]);
-            if constexpr (!USE_P) {
-              const float4 b0 = bb[2 * gq], b1 = bb[2 * gq + 1];
-              r[0] += b0.x; r[1] += b0.y; r[2] += b0.z; r[3] += b0.w; r[4] += b1.x; r[5] += b1.y; r[6] += b1.z; r[7] += b1.w;
-            }
-            if constexpr (USE_H) {
-              if constexpr (H16) {
-                const uint4 hq = cur.h[gq];
-                const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&hq.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&hq.y));
-                const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&hq.z)), f3 = __half22float2(*reinterpret_cast<const __half2*>(&hq.w));
-                r[0] += f0.x; r[1] += f0.y; r[2] += f1.x; r[3] += f1.y; r[4] += f2.x; r[5] += f2.y; r[6] += f3.x; r[7] += f3.y;
-              } else {
-                const uint4 ha = cur.h[2 * gq], hb = cur.h[2 * gq + 1];
-                r[0] += __uint_as_float(ha.x); r[1] += __uint_as_float(ha.y); r[2] += __uint_as_float(ha.z); r[3] += __uint_as_float(ha.w);
-                r[4] += __uint_as_float(hb.x); r[5] += __uint_as_float(hb.y); r[6] += __uint_as_float(hb.z); r[7] += __uint_as_float(hb.w);
-              }
-            }
-            if constexpr (USE_P) {
-              const uint4 pq = cur.p[gq];
-              const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&pq.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&pq.y));
-              const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&pq.z)), f3 = __half22float2(*reinterpret_cast<const __half2*>(&pq.w));
-              r[0] += f0.x; r[1] += f0.y; r[2] += f1.x; r[3] += f1.y; r[4] += f2.x; r[5] += f2.y; r[6] += f3.x; r[7] += f3.y;
-            }
-            if constexpr (WRITE_H) {
-              if constexpr (H16)
-                h8[(size_t)(2 * g + gq) * kTileM] = make_uint4(pack_half2(r[0], r[1]), pack_half2(r[2], r[3]), pack_half2(r[4], r[5]), pack_half2(r[6], r[7]));
-              else {
-                h4[(size_t)(4 * g + 2 * gq) * kTileM] = make_float4(r[0], r[1], r[2], r[3]);
-                h4[(size_t)(4 * g + 2 * gq + 1) * kTileM] = make_float4(r[4], r[5], r[6], r[7]);
-              }
-            }
-            const int gcol = ((col & 63) >> 3) + gq;            // granule inside the 64-wide chunk; swizzle: granule ^ (row & 7)
-            sts128(srow + (uint32_t)(((gcol ^ (erow & 7)) << 4)), pack_relu_half2(r[0], r[1]), pack_relu_half2(r[2], r[3]),
-                   pack_relu_half2(r[4], r[5]), pack_relu_half2(r[6], r[7]));
-          }
-          if (g < 6) load_hp(cur, g + 2);                       // this set's next group
-        };
+      const int g_end = first ? 3 : 8;
 #pragma unroll 1
-        for (int g = 0; g < 8; g += 2) {
-          body(A, B, g);
-          body(B, A, g + 1);
-        }
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0)
-          for (int s_ = 4 * part; s_ < 4 * part + 4; ++s_) arrive_a_full(s_);
-        fill_par ^= 0xFu << (4 * part);
-        lap(WRITE_H ? 3 : (USE_H ? 6 : 5));
-      };
-
-      // ---------------- split mode: the same epilogue for a 64-point tile --------------------------------------------
-      //   TMEM lane r (warps of lane quarters 0,1: "hi warps") holds x_hi W^T, lane r + 64 (quarters 2,3: "lo warps")
-      //   x_lo W^T of the same point; a warp can only read its own lane quarter.  Per group of 16 columns the two warps
-      //   of a pair (same sub, quarters q and q+2) swap halves: the hi warp finishes columns 0-7 and needs the lo warp's
-      //   partial sums of those, the lo warp finishes columns 8-15 and needs the hi warp's.  The 2 x 32 bytes travel
-      //   through exactly the bytes of the next layer's A tile that the RECEIVING lane is about to overwrite with the
-      //   finished operands (granule g or g+1 of rows r and r+64), so no staging buffer exists; one 64-thread named
-      //   barrier per group orders the hand-over.  Both warps then do the same arithmetic on their 8 columns:
-      //   (D_hi + D_lo) * 2^-s + bias (+ h), ReLU, hi/lo split, two 16-byte A-tile stores.
-      //   Flags AND the warp's role (hi / lo lanes) are compile-time, operands of even / odd groups in two register sets.
-      auto epilogue_split_lean = [&](auto mine_c, auto use_h_c, auto write_h_c, auto use_p_c, int part, int bias_idx) __attribute__((always_inline)) {
-        constexpr int MINE = decltype(mine_c)::value;           // 0: hi warp (lanes r), finishes columns 0-7 of a group; 1: lo warp (lanes r+64), 8-15
-        constexpr bool USE_H = decltype(use_h_c)::value, WRITE_H = decltype(write_h_c)::value, USE_P = decltype(use_p_c)::value;
-        lap(1);
-        const int pair_bar = 2 + (q4 & 1) * 2 + sub;            // named barriers 2..5: one per (hi, lo) warp pair
-        const int prow = (q4 & 1) * 32 + lane;                  // point row (0..63) of this lane
-        const float inv_scale = __ldg(bias + kInvScaleSlot);
-        const uint32_t trow = tmem_base + ((uint32_t)(q4 * 32) << 16);
-        const int col0 = part * 256 + sub * 128;
-        const float4* bp = reinterpret_cast<const float4*>(bias + (size_t)bias_idx * kHidden) + (col0 >> 2) + 2 * MINE;          // + 4 per group
-        float4* hp = scratch4 + (size_t)((col0 >> 2) + 2 * MINE) * kTileM + prow;                                              // + 4*kTileM per group
-        const float4* pp4 = reinterpret_cast<const float4*>(pre_row + (size_t)bias_idx * kHidden * 4) + (col0 >> 2) + 2 * MINE;  // + 4 per group
-        struct Set { uint32_t v[16]; float4 h[2]; float4 p[2]; };
-        Set A, B;
-        auto load_hp = [&](Set& s_, int g) __attribute__((always_inline)) {
-          if constexpr (USE_H) { s_.h[0] = hp[(size_t)(4 * g) * kTileM]; s_.h[1] = hp[(size_t)(4 * g + 1) * kTileM]; }
-          if constexpr (USE_P) { s_.p[0] = __ldg(pp4 + 4 * g); s_.p[1] = __ldg(pp4 + 4 * g + 1); }
-        };
-        load_hp(A, 0);
-        load_hp(B, 1);
-        mbar_wait(half_full(part), (half_par >> part) & 1u, a.error_flag);
-        half_par ^= 1u << part;
-        tc_fence_after();
-        lap(2);
-        tmem_ld16(trow + (uint32_t)col0, A.v);
-        auto body = [&](Set& cur, Set& nxt, int g) __attribute__((always_inline)) {
-          const int col = col0 + g * 16;
-          const int slot = col >> 6;
-          if ((g & 3) == 0) wait_slot_free(slot);
-          const uint32_t slot_addr = smem_base + kSmemA + slot * kASlotBytes;
-          const int gcol = (col & 63) >> 3;
-          // mine0/mine1: granule of THIS warp's 8 columns in rows r / r+64 ; peer0/peer1: granule of the partner's columns
-          const uint32_t mine0 = slot_addr + sw128_offset(prow, gcol + MINE), mine1 = slot_addr + sw128_offset(prow + kPts, gcol + MINE);
-          const uint32_t peer0 = slot_addr + sw128_offset(prow, gcol + 1 - MINE), peer1 = slot_addr + sw128_offset(prow + kPts, gcol + 1 - MINE);
-          float4 bb[2];
-          if constexpr (!USE_P) { bb[0] = __ldg(bp + 4 * g); bb[1] = __ldg(bp + 4 * g + 1); }
-          tmem_ld_wait();
-          if (g < 7) tmem_ld16(trow + (uint32_t)(col + 16), nxt.v);
-          // send the 8 partial sums the partner finishes (its columns), keep the other 8
-          constexpr int SND = MINE ? 0 : 8, KEEP = MINE ? 8 : 0;
-          sts128(peer0, cur.v[SND + 0], cur.v[SND + 1], cur.v[SND + 2], cur.v[SND + 3]);
-          sts128(peer1, cur.v[SND + 4], cur.v[SND + 5], cur.v[SND + 6], cur.v[SND + 7]);
-          named_bar_sync(pair_bar, 64);
-          const uint4 p0 = lds128(mine0), p1 = lds128(mine1);
-          const float pr[8] = {__uint_as_float(p0.x), __uint_as_float(p0.y), __uint_as_float(p0.z), __uint_as_float(p0.w),
-                               __uint_as_float(p1.x), __uint_as_float(p1.y), __uint_as_float(p1.z), __uint_as_float(p1.w)};
-          float r[8];
+      for (int g = first ? 0 : 3; g < g_end; ++g) {
+        float v[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            // D_hi + D_lo in this order on both warps (the hi warp holds D_hi, the lo warp receives it)
-            const float own = __uint_as_float(cur.v[KEEP + j]);
-            const float dsum = MINE ? (pr[j] + own) : (own + pr[j]);
-            r[j] = dsum * inv_scale;
-          }
-          if constexpr (!USE_P) {
-            r[0] += bb[0].x; r[1] += bb[0].y; r[2] += bb[0].z; r[3] += bb[0].w; r[4] += bb[1].x; r[5] += bb[1].y; r[6] += bb[1].z; r[7] += bb[1].w;
-          }
-          if constexpr (USE_H) {
-            r[0] += cur.h[0].x; r[1] += cur.h[0].y; r[2] += cur.h[0].z; r[3] += cur.h[0].w;
-            r[4] += cur.h[1].x; r[5] += cur.h[1].y; r[6] += cur.h[1].z; r[7] += cur.h[1].w;
-          }
-          if constexpr (USE_P) {
-            r[0] += cur.p[0].x; r[1] += cur.p[0].y; r[2] += cur.p[0].z; r[3] += cur.p[0].w;
-            r[4] += cur.p[1].x; r[5] += cur.p[1].y; r[6] += cur.p[1].z; r[7] += cur.p[1].w;
-          }
-          if constexpr (WRITE_H) {
-            hp[(size_t)(4 * g) * kTileM] = make_float4(r[0], r[1], r[2], r[3]);
-            hp[(size_t)(4 * g + 1) * kTileM] = make_float4(r[4], r[5], r[6], r[7]);
-          }
+        for (int j = 0; j < 8; ++j) v[j] = xval(8 * g + j, vd);
+        if constexpr (SPLIT) {
           uint32_t hi[4], lo[4];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) split_half2(fmaxf(r[2 * j], 0.0f), fmaxf(r[2 * j + 1], 0.0f), hi[j], lo[j]);
-          sts128(mine0, hi[0], hi[1], hi[2], hi[3]);
-          sts128(mine1, lo[0], lo[1], lo[2], lo[3]);
-          if (g < 6) load_hp(cur, g + 2);
-        };
-#pragma unroll 1
-        for (int g = 0; g < 8; g += 2) {
-          body(A, B, g);
-          body(B, A, g + 1);
-        }
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0)
-          for (int s_ = 4 * part; s_ < 4 * part + 4; ++s_) arrive_a_full(s_);
-        fill_par ^= 0xFu << (4 * part);
-        lap(WRITE_H ? 3 : (USE_H ? 6 : 5));
-      };
-      // run-time (role, use_h, write_h) -> the compile-time variant
-      auto epilogue_split_dispatch = [&](int part, int bias_idx, bool use_h, bool write_h) __attribute__((always_inline)) {
-        using T = std::true_type;
-        using F = std::false_type;
-        using I0 = std::integral_constant<int, 0>;
-        using I1 = std::integral_constant<int, 1>;
-        using P = std::integral_constant<bool, PRE>;
-        if (q4 < 2) {
-          if (write_h) { if (use_h) epilogue_split_lean(I0{}, T{}, T{}, P{}, part, bias_idx); else epilogue_split_lean(I0{}, F{}, T{}, P{}, part, bias_idx); }
-          else { if (use_h) epilogue_split_lean(I0{}, T{}, F{}, F{}, part, bias_idx); else epilogue_split_lean(I0{}, F{}, F{}, F{}, part, bias_idx); }
+          for (int j = 0; j < 4; ++j) split_half2(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
+          sts128(slot_addr + sw128_offset(xrow, g), hi[0], hi[1], hi[2], hi[3]);
+          sts128(slot_addr + sw128_offset(xrow + kPts, g), lo[0], lo[1], lo[2], lo[3]);
         } else {
-          if (write_h) { if (use_h) epilogue_split_lean(I1{}, T{}, T{}, P{}, part, bias_idx); else epilogue_split_lean(I1{}, F{}, T{}, P{}, part, bias_idx); }
-          else { if (use_h) epilogue_split_lean(I1{}, T{}, F{}, F{}, part, bias_idx); else epilogue_split_lean(I1{}, F{}, F{}, F{}, part, bias_idx); }
-        }
-      };
-      auto epilogue = [&](int part, int bias_idx, bool use_h, bool write_h) __attribute__((always_inline)) {
-        using T = std::true_type;
-        using F = std::false_type;
-        if constexpr (SPLIT) epilogue_split_dispatch(part, bias_idx, use_h, write_h);
-        else {
-          // (use_h, write_h) combinations of the tile program: E1 of block 0 (F,T), E1 of blocks 1,2 (T,T), E2 (F,F), E3 (T,F);
-          // the latent table is added in the E1 epilogues only
-          if (write_h) {
-            if (use_h) epilogue_half_lean(T{}, T{}, std::integral_constant<bool, PRE>{}, part, bias_idx);
-            else epilogue_half_lean(F{}, T{}, std::integral_constant<bool, PRE>{}, part, bias_idx);
-          } else {
-            if (use_h) epilogue_half_lean(T{}, F{}, F{}, part, bias_idx);
-            else epilogue_half_lean(F{}, F{}, F{}, part, bias_idx);
-          }
-        }
-      };
-
-      auto dump_acc = [&](bool both_halves) {     // debug: raw accumulator of the current layer
-        mbar_wait(half_full(0), (half_par >> 0) & 1u, a.error_flag);
-        half_par ^= 1u << 0;
-        if (both_halves) { mbar_wait(half_full(1), (half_par >> 1) & 1u, a.error_flag); half_par ^= 1u << 1; }
-        tc_fence_after();
-        for (int grp = 0; grp < 8; ++grp) {
-          const int col = sub * 256 + grp * 32;
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)col, v);
-          tmem_ld_wait();
-          float* dst = a.debug_acc + ((size_t)tile * kTileM + erow) * kHidden + col;   // split mode: rows 64-127 = low-part products
-          if (tile < a.n_tiles) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) dst[j] = __uint_as_float(v[j]);
-          }
-        }
-        tc_fence_before();
-        named_bar_sync(1, kWorkerThreads);
-      };
-
-      // ---------------- the tile program (worker side; MMA side: walk_tile) -------------------------------------
-      lap(0);
-      constexpr bool do_gather = !PRE;                            // latent table: no lin_z chunk exists, nothing to gather or sync
-      if (do_gather) gather_pass(0);                              // lin_z0
-      if (a.debug_layer == 1) { dump_acc(true); continue; }
-      bool stop = false;
-      for (int b = 0; b < SRF_NUM_BLOCKS; ++b) {
-        // one call site per epilogue kind (the bodies are inlined, flags compile-time): the two accumulator halves share the code
-#pragma unroll 1
-        for (int part = 0; part < 2; ++part) epilogue(part, b, b > 0, true);          // E1a, E1b -> A chunks of fc_0
-        if (a.debug_layer == 2 + 3 * b) { dump_acc(true); stop = true; break; }
-#pragma unroll 1
-        for (int part = 0; part < 2; ++part) epilogue(part, 3 + b, false, false);     // E2a (overlaps fc_0 S4), E2b (overlaps fc_1 S1) -> A chunks of fc_1
-        if (b < SRF_NUM_BLOCKS - 1) {
-          if (do_gather) gather_pass(b + 1);                      // lin_z(b+1), consumed between fc_1 S2 and S3
-          if (a.debug_layer == 4 + 3 * b) { dump_acc(true); stop = true; break; }
-        } else {
-          // last block: nothing to gather while fc_1 runs -> prepare the next tile's geometry / chunk mask now
-          if (a.debug_layer < 0 && grp_i + n_cgroups < n_groups) geometry(grp_i + n_cgroups, it + 1);
-          if (a.debug_layer == 9) { dump_acc(true); stop = true; break; }
+          sts128(slot_addr + sw128_offset(xrow, g), pack_half2(v[0], v[1]), pack_half2(v[2], v[3]), pack_half2(v[4], v[5]),
+                 pack_half2(v[6], v[7]));
         }
       }
-      if (stop) continue;
-#pragma unroll 1
-      for (int part = 0; part < 2; ++part) epilogue(part, 6, true, false);            // E3a, E3b -> A chunks of lin_out
-      if (a.debug_layer == 10) { dump_acc(false); continue; }
-      // ---------------- E4: out = ACC[:, :d_out] + b_out ------------------------------------------------------
-      lap(1);
-      mbar_wait(half_full(0), (half_par >> 0) & 1u, a.error_flag);
-      half_par ^= 1u << 0;
-      tc_fence_after();
-      lap(2);
-      if (sub == 0) {
-        uint32_t v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16), v);   // 16 columns
-        tmem_ld_wait();
-        const float* bo = bias + (size_t)7 * kHidden;
+    }
+    fence_proxy_async_smem();
+    sync_all();
+
+    // ---------------- latent gather: chunk c of z into an A chunk -------------------------------------------------
+    // thread -> kItems items per chunk: points (tid/8) + 32*i, granule (8 channels = 16 B of fp16) g = tid % 8.
+    // Per point only (element offset of the north-west tap, x/y fractional weights, 4 validity bits) is kept in
+    // registers for the current scale; the 4 tap weights are re-derived (same products as scale_taps) per chunk.
+    constexpr int kItems = kPts / 32;
+    int cur_scale = -1;
+    int t_off[kItems];          // offset of tap 0 (may be "virtual" when tap 0 itself is out of range)
+    uint32_t t_ok[kItems];      // bit t = tap t in range
+    float t_w[kItems], t_n[kItems];
+    int dxo = 0, dyo = 0;       // element strides to the east / south tap
+    auto gather = [&](int c, uint32_t zaddr) {
+      const int g = tid & 7;
+      const int ch = c * kChunkK + g * 8;                     // first of this thread's 8 channels
+      auto emit_vals = [&](int row, const float (&v)[8]) {
         if constexpr (SPLIT) {
-          // lanes r and r + 64 hold the two halves of the sum: the lo warp passes its 16 values through the (drained)
-          // last A slot; every MMA that read it has completed (EV_OUT is committed after the lin_out MMAs)
-          const int prow = (q4 & 1) * 32 + lane;
-          const uint32_t ex = smem_base + kSmemA + 7 * kASlotBytes + (uint32_t)prow * 64u;
-          if (q4 >= 2) {
+          uint32_t hi[4], lo[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) sts128(ex + 16 * j, v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            named_bar_sync(2 + (q4 & 1) * 2, 64);
-          } else {
-            named_bar_sync(2 + (q4 & 1) * 2, 64);
-            float pl[16];
+          for (int j = 0; j < 4; ++j) split_half2(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
+          sts128(zaddr + sw128_offset(row, g), hi[0], hi[1], hi[2], hi[3]);
+          sts128(zaddr + sw128_offset(row + kPts, g), lo[0], lo[1], lo[2], lo[3]);
+        } else {
+          sts128(zaddr + sw128_offset(row, g), pack_half2(v[0], v[1]), pack_half2(v[2], v[3]), pack_half2(v[4], v[5]), pack_half2(v[6], v[7]));
+        }
+      };
+      int s = -1;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint4 t4 = lds128(ex + 16 * j);
-              pl[4 * j] = __uint_as_float(t4.x); pl[4 * j + 1] = __uint_as_float(t4.y);
-              pl[4 * j + 2] = __uint_as_float(t4.z); pl[4 * j + 3] = __uint_as_float(t4.w);
+      for (int i = 0; i < kScales; ++i)
+        if (ch >= p.ch_off[i] && ch < p.ch_off[i + 1]) s = i;
+      if (s >= 0 && s != cur_scale) {
+        dxo = p.C[s]; dyo = p.W[s] * p.C[s];
+#pragma unroll
+        for (int i = 0; i < kItems; ++i) {
+          const short2 sp16 = sph_cur[(tid >> 3) + 32 * i];
+          const Taps tp = scale_taps(p, s, sp16.x, sp16.y);
+          t_ok[i] = (tp.off[0] >= 0 ? 1u : 0u) | (tp.off[1] >= 0 ? 2u : 0u) | (tp.off[2] >= 0 ? 4u : 0u) | (tp.off[3] >= 0 ? 8u : 0u);
+          // off[t] = off0 + (t&1)*dxo + (t>>1)*dyo for in-range taps -> recover off0 from any valid tap
+          int o0 = 0;
+          if (tp.off[0] >= 0) o0 = tp.off[0];
+          else if (tp.off[1] >= 0) o0 = tp.off[1] - dxo;
+          else if (tp.off[2] >= 0) o0 = tp.off[2] - dyo;
+          else if (tp.off[3] >= 0) o0 = tp.off[3] - dxo - dyo;
+          t_off[i] = o0;
+          t_w[i] = tp.fx; t_n[i] = tp.fy;
+        }
+        cur_scale = s;
+      }
+      const char* fbytes = (s >= 0) ? reinterpret_cast<const char*>(p.feat[s]) : nullptr;
+      const int ch_in = (s >= 0) ? ch - p.ch_off[s] : 0;
+      const bool f16 = p.feat_fp16 != 0;
+#pragma unroll
+      for (int u = 0; u < kItems; ++u) {
+        const int row = (tid >> 3) + 32 * u;
+        float acc[8];
+        const uint32_t ok = (s >= 0) ? t_ok[u] : 0u;
+        if (!ok) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[e] = 0.0f;
+          emit_vals(row, acc);
+          continue;
+        }
+        const float wx = t_w[u], ny = t_n[u];
+        const float e_ = fsub(1.0f, wx), so = fsub(1.0f, ny);
+        const float tw4[4] = {fmul(so, e_), fmul(so, wx), fmul(ny, e_), fmul(ny, wx)};     // nw, ne, sw, se
+        float v[4][8];
+#pragma unroll
+        for (int tp = 0; tp < 4; ++tp) {
+          if ((ok >> tp) & 1u) {
+            const size_t eidx = (size_t)(ch_in + t_off[u] + (tp & 1) * dxo + (tp >> 1) * dyo);
+            if (f16) {
+              const uint4 raw = __ldg(reinterpret_cast<const uint4*>(fbytes + eidx * 2));
+              const uint32_t rw[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&rw[q]));
+                v[tp][2 * q] = f.x; v[tp][2 * q + 1] = f.y;
+              }
+            } else {
+              const float4* src = reinterpret_cast<const float4*>(fbytes + eidx * 4);
+              const float4 a0 = __ldg(src), a1 = __ldg(src + 1);
+              v[tp][0] = a0.x; v[tp][1] = a0.y; v[tp][2] = a0.z; v[tp][3] = a0.w;
+              v[tp][4] = a1.x; v[tp][5] = a1.y; v[tp][6] = a1.z; v[tp][7] = a1.w;
             }
-            const float inv_scale = __ldg(bias + kInvScaleSlot);
-            const int gi = row0 + prow;
-            if (gi < a.n) {
+          } else {
 #pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (j < a.d_out) a.raw_out[(size_t)gi * a.d_out + j] = (__uint_as_float(v[j]) + pl[j]) * inv_scale + __ldg(bo + j);
+            for (int e = 0; e < 8; ++e) v[tp][e] = 0.0f;
+          }
+        }
+        // out = ((v_nw*nw + v_ne*ne) + v_sw*sw) + v_se*se : separate roundings like ATen's CPU kernel
+        // (an out-of-range tap contributes an exact +0)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          acc[e] = fmul(v[0][e], tw4[0]);
+#pragma unroll
+          for (int tp = 1; tp < 4; ++tp) acc[e] = fadd(acc[e], fmul(v[tp][e], tw4[tp]));
+        }
+        emit_vals(row, acc);
+      }
+    };
+    // one lin_z layer: the active chunks in order, chunk i+1 gathered while the MMAs of chunk i run
+    auto zpass = [&]() {
+      cur_scale = -1;
+      int c = next_active(kz, mask, -1);
+      if (c < 0) return;
+      gather(c, smem_base + kSmemZ);
+      fence_proxy_async_smem();
+      sync_all();
+      for (int zi = 0; c >= 0; ++zi) {
+        const int cn = next_active(kz, mask, c);
+        mma_pair(smem_base + kSmemZ + (uint32_t)(zi & 1) * kAChunkBytes, false);
+        if (cn >= 0) gather(cn, smem_base + kSmemZ + (uint32_t)((zi + 1) & 1) * kAChunkBytes);
+        retire0();
+        fence_proxy_async_smem();
+        sync_all();
+        c = cn;
+      }
+    };
+
+    // ---------------- epilogue of the warpgroup's 256 columns: registers -> [+bias (+h) (+table)] -> A = relu -------
+    //   register i of accumulator j: row erow0 + 8 ((i/2) % 2), column 256 wg + 128 j + 8 (i/4) + ecol + (i % 2)
+    //   h is kept in register order: element (j, i) of thread t at hbuf[(j * 64 + i) * 128 + t]
+    auto epilogue = [&](auto use_h_c, auto write_h_c, auto use_p_c, int bias_idx) __attribute__((always_inline)) {
+      constexpr bool USE_H = decltype(use_h_c)::value, WRITE_H = decltype(write_h_c)::value, USE_P = decltype(use_p_c)::value;
+      if constexpr (SPLIT) {
+        // low-part sums (rows 32-63, threads 64-127 of the warpgroup) go to the thread 64 below
+        if (t >= 64) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) { xbuf[i * 64 + (t - 64)] = acc0[i]; xbuf[(64 + i) * 64 + (t - 64)] = acc1[i]; }
+        }
+        named_bar_sync(2 + wg, 128);
+        if (t >= 64) return;
+      }
+      [[maybe_unused]] const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
+      auto finish = [&](float (&acc)[64], int j) __attribute__((always_inline)) {
+#pragma unroll
+        for (int i2 = 0; i2 < 32; ++i2) {
+          const int i = 2 * i2, hh = i2 & 1;
+          const int row = erow0 + 8 * hh;
+          const int col = 256 * wg + 128 * j + 8 * (i2 >> 1) + ecol;
+          float r0 = acc[i], r1 = acc[i + 1];
+          if constexpr (SPLIT) {
+            const float p0 = xbuf[(j * 64 + i) * 64 + t], p1 = xbuf[(j * 64 + i + 1) * 64 + t];
+            r0 = (r0 + p0) * inv_scale; r1 = (r1 + p1) * inv_scale;      // D_hi + D_lo
+          }
+          if constexpr (!USE_P) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + (size_t)bias_idx * kHidden + col));
+            r0 += bb.x; r1 += bb.y;
+          }
+          [[maybe_unused]] float2* hp = reinterpret_cast<float2*>(hbuf) + (size_t)(j * 32 + i2) * 128 + t;
+          [[maybe_unused]] __half2* hp16 = reinterpret_cast<__half2*>(hbuf) + (size_t)(j * 32 + i2) * 128 + t;
+          if constexpr (USE_H) {
+            if constexpr (H16) { const float2 f = __half22float2(*hp16); r0 += f.x; r1 += f.y; }
+            else { const float2 f = *hp; r0 += f.x; r1 += f.y; }
+          }
+          if constexpr (USE_P) {
+            if constexpr (SPLIT) {
+              const float2 f = __ldg(reinterpret_cast<const float2*>(pre_row[hh] + ((size_t)bias_idx * kHidden + col) * 4));
+              r0 += f.x; r1 += f.y;
+            } else {
+              const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2*>(pre_row[hh] + ((size_t)bias_idx * kHidden + col) * 2)));
+              r0 += f.x; r1 += f.y;
             }
           }
+          if constexpr (WRITE_H) {
+            if constexpr (H16) *hp16 = __floats2half2_rn(r0, r1);
+            else *hp = make_float2(r0, r1);
+          }
+          const uint32_t addr = smem_base + kSmemAct + (uint32_t)(col >> 6) * kAChunkBytes;
+          const uint32_t inrow = (uint32_t)((((col & 63) >> 3) ^ (row & 7)) << 4) + (uint32_t)((col & 7) * 2);
+          if constexpr (SPLIT) {
+            uint32_t hi, lo;
+            split_half2(fmaxf(r0, 0.0f), fmaxf(r1, 0.0f), hi, lo);
+            sts32(addr + (uint32_t)row * 128 + inrow, hi);
+            sts32(addr + (uint32_t)(row + kPts) * 128 + inrow, lo);
+          } else {
+            sts32(addr + (uint32_t)row * 128 + inrow, pack_relu_half2(r0, r1));
+          }
+        }
+      };
+      finish(acc0, 0);
+      finish(acc1, 1);
+    };
+    // epilogue boundary: every MMA of both warpgroups that reads the A tile has completed before it is overwritten,
+    // and the new tile is visible to the async proxy before the next layer's MMAs
+    auto epi = [&](auto use_h_c, auto write_h_c, auto use_p_c, int bias_idx) __attribute__((always_inline)) {
+      retire0();
+      sync_all();
+      epilogue(use_h_c, write_h_c, use_p_c, bias_idx);
+      fence_proxy_async_smem();
+      sync_all();
+    };
+    auto dump_acc = [&](bool out) {     // debug: raw accumulator of the current layer
+      retire0();
+      if (out && wg != 0) return;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float* dst = a.debug_acc + ((size_t)tile * kTileM + erow0 + 8 * hh) * kHidden;   // split mode: rows 32-63 = low-part products
+        if (out) {
+#pragma unroll
+          for (int c8 = 0; c8 < 2; ++c8) { dst[8 * c8 + ecol] = acco[4 * c8 + 2 * hh]; dst[8 * c8 + ecol + 1] = acco[4 * c8 + 2 * hh + 1]; }
         } else {
-          const int gi = row0 + erow;
-          if (gi < a.n) {
-            for (int j = 0; j < a.d_out; ++j) a.raw_out[(size_t)gi * a.d_out + j] = __uint_as_float(v[j]) + __ldg(bo + j);
+#pragma unroll
+          for (int c8 = 0; c8 < 16; ++c8) {
+            const int col = 256 * wg + 8 * c8 + ecol;
+            dst[col] = acc0[4 * c8 + 2 * hh]; dst[col + 1] = acc0[4 * c8 + 2 * hh + 1];
+            dst[col + 128] = acc1[4 * c8 + 2 * hh]; dst[col + 129] = acc1[4 * c8 + 2 * hh + 1];
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      lap(3);
-    }
-    if constexpr (PROF) if (prof_on) {
-      unsigned long long* dst = a.prof + (size_t)blockIdx.x * 16;
-      for (int i = 0; i < 4; ++i) dst[i] = (unsigned long long)pc[i];
-      dst[4] = (unsigned long long)(clock64() - pt_start);
-      dst[5] = (unsigned long long)pc[5]; dst[6] = (unsigned long long)pc[6]; dst[7] = (unsigned long long)pc[7];
-    }
-  }
+    };
 
-  // ---- teardown -------------------------------------------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (CG == 2) cluster_sync_all();           // no CTA may exit while its peer can still signal its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<CG>(tmem_base, kTmemCols);
+    // ---------------- the tile program ---------------------------------------------------------------------------
+    using T = std::true_type;
+    using F = std::false_type;
+    using P = std::integral_constant<bool, PRE>;
+    mma_pair(smem_base + kSmemX, true);                           // lin_in
+    retire1();
+    if (!PRE) zpass();                                            // lin_z0
+    if (a.debug_layer == 1) { dump_acc(false); continue; }
+    bool stop = false;
+    for (int b = 0; b < SRF_NUM_BLOCKS; ++b) {
+      if (b == 0) epi(F{}, T{}, P{}, b);                          // E1 -> A = relu(h)
+      else epi(T{}, T{}, P{}, b);
+#pragma unroll 1
+      for (int k = 0; k < kHiddenChunks; ++k) { mma_pair(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // fc_0
+      if (a.debug_layer == 2 + 3 * b) { dump_acc(false); stop = true; break; }
+      epi(F{}, F{}, F{}, 3 + b);                                  // E2 -> A = relu(net)
+#pragma unroll 1
+      for (int k = 0; k < kHiddenChunks; ++k) { mma_pair(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // fc_1
+      if (b < SRF_NUM_BLOCKS - 1) {
+        if (!PRE) zpass();                                        // lin_z(b+1) accumulates onto fc_1
+        if (a.debug_layer == 4 + 3 * b) { dump_acc(false); stop = true; break; }
+      } else if (a.debug_layer == 9) { dump_acc(false); stop = true; break; }
+    }
+    if (stop) continue;
+    epi(T{}, F{}, F{}, 6);                                        // E3 -> A = relu(h)
+    if (wg == 0) {
+#pragma unroll 1
+      for (int k = 0; k < kHiddenChunks; ++k) { mma_out(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // lin_out
+      if (a.debug_layer == 10) { dump_acc(true); continue; }
+      retire0();
+      // ---------------- E4: out = ACC[:, :d_out] + b_out ------------------------------------------------------
+      const float* bo = bias + (size_t)7 * kHidden;
+      if constexpr (SPLIT) {
+        if (t >= 64) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) xbuf[i * 64 + (t - 64)] = acco[i];
+        }
+        named_bar_sync(2, 128);
+      }
+      if (!SPLIT || t < 64) {
+        const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int row = erow0 + 8 * ((i >> 1) & 1);
+          const int col = 8 * (i >> 2) + ecol + (i & 1);
+          float v = acco[i];
+          if constexpr (SPLIT) v = (v + xbuf[i * 64 + t]) * inv_scale;
+          const int gi = row0 + row;
+          if (row < kPts && gi < a.n && col < a.d_out) a.raw_out[(size_t)gi * a.d_out + col] = v + __ldg(bo + col);
+        }
+      }
+    }
   }
 }
 
@@ -1597,80 +881,24 @@ static int* g_wd_host = nullptr;
 static int* g_wd_dev = nullptr;
 int tc_watchdog_flag() { return g_wd_host ? *g_wd_host : 0; }
 
-static int g_num_sms = 0;
-static int num_sms() {
-  if (!g_num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
-  }
-  return g_num_sms;
-}
+static int num_sms() { return device_sm_count(); }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time dependency on libcuda)
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-// [rows x 64] fp16 row-major (128 B rows, already in shared-memory byte order), box = box_rows x 64
-static bool encode_image_map(CUtensorMap* tm, void* base, size_t rows, int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn || rows == 0) return false;
-  const cuuint64_t dims[2] = {64, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {128};
-  const cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-static bool tc_use_tmap() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("SRF_TC_TMAP"); v = (e && atoi(e) == 0) ? 0 : 1; }
-  return v == 1;
-}
-
-using TcKernelFn = void (*)(const DevParams, const tc::KernelArgs, const CUtensorMap, const CUtensorMap);
-constexpr int kNumTcKernels = 24;
-// index: bit 0 = CTA pairs, bit 1 = profiling counters, then 0 = fp32 hidden state, 4 = fp16 hidden state, 8 = split mode; +12 = latent table
-#define SRF_TC_ROW(H16_, SPLIT_, PRE_)                                                                              \
-  tc::point_mlp_tc_kernel<1, false, H16_, SPLIT_, PRE_>, tc::point_mlp_tc_kernel<2, false, H16_, SPLIT_, PRE_>,     \
-  tc::point_mlp_tc_kernel<1, true, H16_, SPLIT_, PRE_>, tc::point_mlp_tc_kernel<2, true, H16_, SPLIT_, PRE_>
+using TcKernelFn = void (*)(const DevParams, const tc::KernelArgs);
+constexpr int kNumTcKernels = 6;
+// index: 0 = fp32 hidden state, 1 = fp16 hidden state, 2 = split mode; +3 = latent table
 static TcKernelFn tc_kernel_at(int i) {
   static const TcKernelFn table[kNumTcKernels] = {
-      SRF_TC_ROW(false, false, false), SRF_TC_ROW(true, false, false), SRF_TC_ROW(false, true, false),
-      SRF_TC_ROW(false, false, true),  SRF_TC_ROW(true, false, true),  SRF_TC_ROW(false, true, true)};
+      tc::point_mlp_tc_kernel<false, false, false>, tc::point_mlp_tc_kernel<true, false, false>, tc::point_mlp_tc_kernel<false, true, false>,
+      tc::point_mlp_tc_kernel<false, false, true>,  tc::point_mlp_tc_kernel<true, false, true>,  tc::point_mlp_tc_kernel<false, true, true>};
   return table[i];
 }
-static TcKernelFn tc_kernel(int cg, bool prof, bool h16, bool split, bool pre = false) {
-  return tc_kernel_at((cg == 2 ? 1 : 0) | (prof ? 2 : 0) | (split ? 8 : (h16 ? 4 : 0)) + (pre ? 12 : 0));
-}
+static TcKernelFn tc_kernel(bool h16, bool split, bool pre) { return tc_kernel_at((split ? 2 : (h16 ? 1 : 0)) + (pre ? 3 : 0)); }
 
-static int tc_cta_group() {
-  static int cg = -1;
-  if (cg < 0) {
-    const char* e = getenv("SRF_TC_CTA_GROUP");
-    cg = (e && atoi(e) == 1) ? 1 : 2;
-  }
-  return cg;
-}
-
+constexpr int kMaxTcCtas = 256;
 size_t tc_workspace_bytes(int d_latent, int n_points) {
   (void)d_latent; (void)n_points;
-  // h scratch for up to 256 CTAs + latent-chunk cache + slack
-  return (size_t)256 * tc::kTileM * kHidden * sizeof(float) + (size_t)256 * tc::kZCache * tc::kASlotBytes + 256;
+  // hidden-state / hand-over scratch for up to kMaxTcCtas CTAs + slack
+  return (size_t)kMaxTcCtas * tc::kScratchFloats * sizeof(float) + 256;
 }
 
 int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n,
@@ -1678,20 +906,18 @@ int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const f
                            int debug_layer, float* debug_acc, cudaStream_t st) {
   if (ws_bytes < tc_workspace_bytes(p.d_latent, n)) return -1;
   if (debug_layer >= 0 && !(debug_layer < tc::kNumLayers && debug_layer != 0 && debug_layer != 3 && debug_layer != 6))
-    return -2;                         // layers without an ACC-complete signal cannot be dumped
+    return -2;                         // layers without an accumulator-complete point cannot be dumped
+  const size_t smem = tc::kSmemTotal + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    for (int i = 0; i < kNumTcKernels; ++i)
-      cudaFuncSetAttribute(tc_kernel_at(i), cudaFuncAttributeMaxDynamicSharedMemorySize, tc::kSmemTotal + 1024);
+    for (int i = 0; i < kNumTcKernels; ++i) cudaFuncSetAttribute(tc_kernel_at(i), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr_set = true;
   }
   const bool split = (flags & kTcFlagSplit) != 0;
-  const int parts = split ? 2 : 1;
   const int tile_pts = split ? tc::kTileM / 2 : tc::kTileM;
   tc::KernelArgs a;
   a.pts = pts; a.viewdir = viewdir; a.n = n; a.n_per = n_per;
   a.n_tiles = (n + tile_pts - 1) / tile_pts;
-  a.split = split ? 1 : 0;
   a.kz = kz_of(p.d_latent);
   a.wblob = reinterpret_cast<const unsigned char*>(split ? w.tc_split_packed : w.tc_packed);
   if (!a.wblob) return -3;
@@ -1707,8 +933,6 @@ int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const f
     a.skip_zero = 0;
   }
   a.debug_layer = debug_layer; a.debug_acc = debug_acc;
-  a.zcache = reinterpret_cast<unsigned char*>(workspace) + (size_t)256 * tc::kTileM * kHidden * sizeof(float);
-  if (const char* e = getenv("SRF_TC_ZCACHE")) { if (atoi(e) == 0) a.zcache = nullptr; }
   // watchdog flag in mapped pinned host memory: still readable after a device-side trap killed the context
   if (!g_wd_host) {
     if (cudaHostAlloc(reinterpret_cast<void**>(&g_wd_host), sizeof(int), cudaHostAllocMapped) == cudaSuccess) {
@@ -1717,64 +941,11 @@ int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const f
     }
   }
   a.error_flag = g_wd_dev;
-  static const bool prof_env = getenv("SRF_TC_PROF") != nullptr;
-  static unsigned long long* prof_dev = nullptr;
-  a.prof = nullptr;
-  if (prof_env) {
-    if (!prof_dev) cudaMalloc(&prof_dev, 256 * 16 * sizeof(unsigned long long));
-    cudaMemsetAsync(prof_dev, 0, 256 * 16 * sizeof(unsigned long long), st);
-    a.prof = prof_dev;
-  }
-  // CTA pairs (cta_group::2, cluster of 2) by default; SRF_TC_CTA_GROUP=1 selects the single-CTA variant.
-  const int cg = (tc_cta_group() == 2 && a.n_tiles >= 2) ? 2 : 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(tc::kThreads);
-  cfg.dynamicSmemBytes = tc::kSmemTotal + 1024;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cg; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  int max_ctas = num_sms();
-  if (cg == 2) {
-    static int max_pairs = 0;
-    if (!max_pairs) {
-      cfg.gridDim = dim3(num_sms() / 2 * 2);
-      int nc = 0;
-      if (cudaOccupancyMaxActiveClusters(&nc, tc_kernel(2, false, false, false), &cfg) != cudaSuccess || nc < 1) nc = num_sms() / 2;
-      max_pairs = nc;
-    }
-    max_ctas = max_pairs * 2;
-  }
-  const int n_groups = (a.n_tiles + cg - 1) / cg;
-  int grid = n_groups * cg < max_ctas ? n_groups * cg : max_ctas;
-  if (grid > 256) grid = 256;
-  cfg.gridDim = dim3(grid);
-  // tensor maps over the weight-image region of the blob (pair mode): [rows x 64] fp16, box = one stage image
-  CUtensorMap tm_main, tm_out;
-  memset(&tm_main, 0, sizeof(tm_main));
-  memset(&tm_out, 0, sizeof(tm_out));
-  a.use_tmap = 0;
-  if (cg == 2 && tc_use_tmap()) {
-    const size_t img_bytes = tc::images_bytes(a.kz, parts);
-    unsigned char* img = const_cast<unsigned char*>(a.wblob) + tc::kHeaderBytes;
-    const size_t out_bytes = (size_t)tc::kHiddenChunks * tc::kOutImgBytes * parts;
-    if (encode_image_map(&tm_main, img, (img_bytes - out_bytes) / 128, tc::kBRows) &&
-        encode_image_map(&tm_out, img + (img_bytes - out_bytes), out_bytes / 128, tc::kOutN / 2))
-      a.use_tmap = 1;
-  }
-  cudaLaunchKernelEx(&cfg, tc_kernel(cg, prof_env, a.hidden_fp16 != 0, split, a.preproj != nullptr), p, a, tm_main, tm_out);
-  if (prof_env) {            // diagnostics only: synchronises and prints mean per-CTA cycle counters
-    static unsigned long long host[256 * 16];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(host, prof_dev, sizeof(host), cudaMemcpyDeviceToHost);
-    double m[16] = {0};
-    for (int b = 0; b < grid; ++b) for (int i = 0; i < 16; ++i) m[i] += (double)host[b * 16 + i] / grid;
-    const double tiles = (double)((n_groups + grid / cg - 1) / (grid / cg));
-    fprintf(stderr, "[srf tc prof] cg=%d grid=%d tiles/CTA=%.0f  per-tile kcycles: total %.1f | worker: front %.1f gather %.1f (blocked on slots %.1f) wait_acc %.1f epi E1x3 %.1f E2x3 %.1f E3 %.1f | issuer(leader avg x%d): wait_A %.1f wait_B %.1f\n",
-            cg, grid, tiles, m[4] / tiles / 1e3, m[0] / tiles / 1e3, m[1] / tiles / 1e3, m[7] / tiles / 1e3, m[2] / tiles / 1e3,
-            m[3] / tiles / 1e3, m[5] / tiles / 1e3, m[6] / tiles / 1e3, cg, m[8] * cg / tiles / 1e3, m[9] * cg / tiles / 1e3);
-  }
+  // persistent: one CTA per SM (the shared-memory footprint allows no second one), tiles round-robin
+  int grid = a.n_tiles < num_sms() ? a.n_tiles : num_sms();
+  if (grid > kMaxTcCtas) grid = kMaxTcCtas;
+  if (grid < 1) return 0;                       // no point: nothing launched
+  tc_kernel(a.hidden_fp16 != 0, split, a.preproj != nullptr)<<<grid, tc::kThreads, smem, st>>>(p, a);
   return 1;
 }
 

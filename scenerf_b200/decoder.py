@@ -1,7 +1,7 @@
 """Producer tail of the feature pyramid on the device: the convolutional part of `DecoderSphere.forward`
 (/root/reference/scenerf/models/unet2d_sphere.py:167-206) -- six `get_sphere_feature` resamplings (csrc/sphere_feature.cu) and the
 five `UpSampleBN` stacks (:37-57: bilinear align_corners upsample + concat, Conv2d 3x3, three dilated `BasicBlock`s with eval-mode
-BatchNorm, LeakyReLU and residual add) as tcgen05 kind::tf32 implicit GEMMs on channels-last maps (csrc/conv_tf32.cu).
+BatchNorm, LeakyReLU and residual add) as wgmma tf32 implicit GEMMs on channels-last maps (csrc/conv_tf32.cu).
 
 The last convolution of every level writes its [H][W][C] output straight into one contiguous buffer laid out exactly like
 `srf_pack_pyramid`'s result (fp32 and, optionally, fp16): `PackedPyramid` is handed to `B200Renderer.render_rays_batch` /

@@ -71,7 +71,7 @@ class _PackedMlp:
 
 
 class B200Renderer:
-    """Drop-in for the renderer half of SceneRF (scenerf.py:392-748) on one B200.
+    """Drop-in for the renderer half of SceneRF (scenerf.py:392-748) on one H100.
 
     hp: dict with the module attributes the path reads -- dataset ("kitti"|"bf"), n_pts_uni, n_gaussians,
         n_pts_per_gaussian, std, max_sample_depth, out_img_W, out_img_H, som_sigma, v_angle_min/max,
@@ -404,7 +404,7 @@ class B200Renderer:
         return g.value, m.value
 
     def debug_tc_layer(self, mlp, cam_pts, x_rgb, cam_K, viewdir, layer: int):
-        """Diagnostic: raw fp32 TMEM accumulator (ceil(n/128)*128, 512) after `layer` of the tensor-core tile
+        """Diagnostic: raw fp32 accumulator (ceil(n/tile)*64, 512; tile = 64 points, 32 in fp32tc) after `layer` of the tensor-core tile
         program (include/scenerf_b200.h: srf_debug_tc_layer)."""
         net = self._select(mlp)
         if net.packed is None and net.packed_split is None:
@@ -415,8 +415,8 @@ class B200Renderer:
         cfg = self._config(cam_K, None)
         pyr = self._pack_pyramid(x_rgb, cfg)
         n = n_cols * n_per
-        tile = 64 if self.precision == "fp32tc" else 128
-        acc = torch.zeros(((n + tile - 1) // tile * 128, 512), dtype=torch.float32, device=self.device)
+        tile = 32 if self.precision == "fp32tc" else 64
+        acc = torch.zeros(((n + tile - 1) // tile * 64, 512), dtype=torch.float32, device=self.device)
         ws = self._workspace(self.lib.srf_predict_workspace_bytes(C.byref(cfg), n))
         _lib.check(self.lib.srf_debug_tc_layer(C.byref(cfg), C.byref(pyr), C.byref(net.struct), _ptr(pts), _ptr(vd),
                                                n_cols, n_per, int(layer), _ptr(acc), _ptr(ws), ws.numel(),
@@ -437,7 +437,7 @@ class B200Renderer:
 
 
 def patch(model, **kw):
-    """Replace `model.render_rays_batch` / `model.predict` of a reference SceneRF module by the B200 path.
+    """Replace `model.render_rays_batch` / `model.predict` of a reference SceneRF module by the CUDA path.
     Call again after loading new weights.  Returns the renderer."""
     r = B200Renderer.from_module(model, **kw)
     if r.hp["dataset"] == "kitti":

@@ -223,7 +223,7 @@ def _full_tensor_check(tensors, ref, what, l2_max, cos_min):
 
 
 def test_tf32_emulation_sets_the_tolerance():
-    """CPU: the float64 oracle with tf32-truncated GEMM operands (what tcgen05 kind::tf32 feeds the multipliers) against the
+    """CPU: the float64 oracle with tf32-truncated GEMM operands (what wgmma .tf32 feeds the multipliers) against the
     exact float64 oracle.  This is the deviation ANY tf32 implementation shows on these small cases (<= 3072 points, so a few
     hundred ReLU-derivative flips are visible): full-tensor relative L2 up to 0.10, cosine >= 0.995.  The GPU test below
     holds the CUDA tf32 mode to 2x that."""
@@ -247,7 +247,7 @@ def test_tf32_emulation_sets_the_tolerance():
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_cuda_backward_tf32_mode(name):
-    """matmul="tf32": the GEMMs of forward and backward on tcgen05 kind::tf32 (float32 storage, 10-bit mantissa operands,
+    """matmul="tf32": the GEMMs of forward and backward on wgmma .tf32 (float32 storage, 10-bit mantissa operands,
     float32 accumulate).  Bounds from the emulation above: loss 2e-3 relative, depth 1.5e-3 * max_sample_depth, every
     gradient tensor within relative L2 0.2 / cosine 0.98 of the exact (float64) gradient.  The strict float32 mode keeps the
     tight bounds of the tests above."""

@@ -1,10 +1,10 @@
 """GPU: the float32-grade tensor-core mode (precision="fp32tc", SRF_PREC_FP32_TC).
 
-Every fp32 operand of the ResnetFC GEMMs (resnetfc.py:54-63,133-164) is carried as an fp16 hi/lo pair; the tile holds 64
-points whose high parts are MMA rows 0-63 and low parts rows 64-127, every weight image is followed by the image of its
-low parts, and the epilogue adds TMEM lanes r and r+64.  Checked here:
+Every fp32 operand of the ResnetFC GEMMs (resnetfc.py:54-63,133-164) is carried as an fp16 hi/lo pair; the tile holds 32
+points whose high parts are MMA rows 0-31 and low parts rows 32-63, every weight image is followed by the image of its
+low parts, and the epilogue adds accumulator rows r and r+32.  Checked here:
   * layer by layer against a float64 evaluation of the UNROUNDED operands (the raw accumulator dump is recombined as
-    (D[r] + D[r+64]) / 2^s) -- localises a wrong image order / scale / lane pairing to the layer;
+    (D[r] + D[r+32]) / 2^s) -- localises a wrong image order / scale / lane pairing to the layer;
   * against the strict fp32 SIMT path on many tiles with a ragged tail, at float32 round-off tolerance;
   * zero-chunk skipping stays bit-identical; ragged batches are bit-equal to the prefix of the full batch.
 Golden parity of the whole render at the fp32 tolerances is in test_gpu_parity.py (precision "fp32tc")."""
@@ -60,7 +60,7 @@ def test_split_tile_program_layer_by_layer(which):
     import torch
     cfg, seed = PREDICT_CASES["predict_adversarial_kitti"]
     g = load_golden("predict_adversarial_kitti")
-    pts, vd = g["cam_pts"][:41], g["viewdir"][:41]        # 328 points: 5 tiles of 64 + a ragged one of 8
+    pts, vd = g["cam_pts"][:41], g["viewdir"][:41]        # 328 points: 10 tiles of 32 + a ragged one of 8
     pm, pg = params_for(cfg)
     params = pm if which == "mlp" else pg
     exp = exact_layers(cfg, params, pts, vd, pyramid_for(cfg, seed))
@@ -75,7 +75,7 @@ def test_split_tile_program_layer_by_layer(which):
     for layer in (1, 2, 4, 5, 7, 8, 9, 10):
         acc = r.debug_tc_layer(which, torch.from_numpy(pts), x_rgb, K, torch.from_numpy(vd), layer)
         torch.cuda.synchronize()
-        raw = acc.cpu().numpy().astype(np.float64).reshape(-1, 2, 64, 512)        # (tile, hi/lo part, row, col)
+        raw = acc.cpu().numpy().astype(np.float64).reshape(-1, 2, 32, 512)        # (tile, hi/lo part, row, col)
         got = ((raw[:, 0] + raw[:, 1]) * inv).reshape(-1, 512)[:n]
         want = exp[layer]
         ncol = want.shape[1]
@@ -85,7 +85,7 @@ def test_split_tile_program_layer_by_layer(which):
         print("%s layer %2d: max|acc| %.3e  max-abs-err %.3e (rel %.1e), low-part rows / high-part rows %.1e"
               % (which, layer, mag, err, err / mag, lo_share))
         assert err <= 2e-5 * mag + 1e-6, "layer %d: err %.3e (scale %.3e)" % (layer, err, mag)
-        assert lo_share < 2e-3                                 # rows 64..127 really are the 2^-11-sized low parts
+        assert lo_share < 2e-3                                 # rows 32..63 really are the 2^-11-sized low parts
     raw = r.predict(which, torch.from_numpy(pts), x_rgb, K, None, torch.from_numpy(vd), output_type="offset")
     got = raw.reshape(n, -1).cpu().numpy()
     want = exp["final"]
@@ -93,7 +93,7 @@ def test_split_tile_program_layer_by_layer(which):
 
 
 def test_fp32tc_vs_fp32_device_paths_large_ragged():
-    """split tensor-core path against the strict fp32 SIMT path on the device: 327 tiles of 64 + ragged tail."""
+    """split tensor-core path against the strict fp32 SIMT path on the device: 653 tiles of 32 + ragged tail."""
     import torch
     from scenerf_b200 import synth
     cfg, seed = RENDER_CASES["kitti_mini"]

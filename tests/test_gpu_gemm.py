@@ -1,5 +1,5 @@
 """The two GEMM kernels of the training path against float64 matmul (through the C ABI: srf_debug_gemm).
-float32 SIMT: round-off (1e-5 of the row/column norms); tcgen05 kind::tf32: 10-bit mantissa operands, bound 2e-3."""
+float32 SIMT: round-off (1e-5 of the row/column norms); wgmma .tf32: 10-bit mantissa operands, bound 2e-3."""
 import ctypes as C
 
 import numpy as np

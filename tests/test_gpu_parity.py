@@ -1,11 +1,11 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  The CUDA path is called through the C ABI (via the ctypes
+"""GPU parity tests (run on an H100: pytest -m gpu).  The CUDA path is called through the C ABI (via the ctypes
 binding) on the same seeded inputs + recorded noise as the reference goldens and compared with
   * the goldens themselves (outputs of the unmodified reference, tests/golden/make_goldens.py), and
   * the CPU oracle for sizes/configs the goldens do not cover.
 Stated tolerances (also in DESIGN.md):
   fp32 (SIMT) mode   : float32 round-off, abs <= 2e-6 + 2e-4 * max(1, |ref|max)
-  fp32tc (tcgen05)   : fp16 hi/lo split operands, fp32 accumulate -- float32-grade: the SAME tolerances as fp32
-  fp16 (tcgen05)     : fp16 operands / fp32 accumulate ("fast mode"): depth <= 3e-4 * max_sample_depth (3 cm of 100 m),
+  fp32tc (wgmma)     : fp16 hi/lo split operands, fp32 accumulate -- float32-grade: the SAME tolerances as fp32
+  fp16 (wgmma)       : fp16 operands / fp32 accumulate ("fast mode"): depth <= 3e-4 * max_sample_depth (3 cm of 100 m),
                        colour <= 1e-3, other per-sample quantities <= 1e-2 * max(1, |ref|max)
 Discrete decisions (rounded sphere pixel, arg-min sample, SOM best-matching unit) are compared exactly where the
 implementations agree on the decision and counted where a last-ulp difference flips it."""

@@ -1,5 +1,5 @@
-"""GPU: the tcgen05 tile program checked layer by layer.  After each accumulator-complete point of the fused kernel
-the raw fp32 TMEM accumulator is dumped (srf_debug_tc_layer) and compared with a float64 emulation that applies the
+"""GPU: the wgmma tile program checked layer by layer.  After each accumulator-complete point of the fused kernel
+the raw fp32 accumulator is dumped (srf_debug_tc_layer) and compared with a float64 emulation that applies the
 same fp16 operand rounding (oracle geometry / gather / positional encoding + numpy matmuls).  This localises a wrong
 shared-memory descriptor, swizzle, weight image or epilogue to the exact layer."""
 import numpy as np
@@ -58,7 +58,7 @@ def test_tile_program_layer_by_layer(which):
     import torch
     cfg, seed = PREDICT_CASES["predict_adversarial_kitti"]
     g = load_golden("predict_adversarial_kitti")
-    pts, vd = g["cam_pts"][:41], g["viewdir"][:41]        # 41 x 8 = 328 points: 3 tiles, last one ragged
+    pts, vd = g["cam_pts"][:41], g["viewdir"][:41]        # 41 x 8 = 328 points: 6 tiles of 64, last one ragged
     pm, pg = params_for(cfg)
     params = pm if which == "mlp" else pg
     exp = emulate(cfg, params, pts, vd, pyramid_for(cfg, seed))
@@ -83,13 +83,13 @@ def test_tile_program_layer_by_layer(which):
 
 
 def test_fp16_vs_fp32_device_paths_large_ragged():
-    """tensor-core path against the strict fp32 SIMT path on the device, many tiles + ragged tail + >148 tiles."""
+    """tensor-core path against the strict fp32 SIMT path on the device, many tiles + ragged tail + more tiles than SMs."""
     import torch
     from scenerf_b200 import synth
     cfg, seed = RENDER_CASES["kitti_mini"]
     x_rgb = torch_pyramid(cfg, seed)
     K = torch.from_numpy(cfg.K)
-    n_cols, n_per = 2611, 8                                   # 20888 points = 163 tiles + 24 rows
+    n_cols, n_per = 2611, 8                                   # 20888 points = 326 tiles of 64 + 24 rows
     u = synth.hash_uniform(91, n_cols * n_per * 3).reshape(n_cols, n_per, 3)
     pts = np.stack([u[..., 0] * 25, u[..., 1] * 4, u[..., 2] * 45 + 46], axis=-1).astype(np.float32)
     vd = (synth.hash_uniform(92, n_cols * 3).reshape(n_cols, 3) * 0.7).astype(np.float32)
