@@ -246,6 +246,26 @@ int srf_tsdf_integrate(float* tsdf_dev, float* weight_dev, float* color_dev, con
 int srf_tsdf_merge(float* tsdf_a, float* weight_a, float* color_a, const float* tsdf_b, const float* weight_b,
                    const float* color_b, const int* dims, void* stream);
 
+/* --- next row: mesh extraction from the fused volume ---------------------------------------------------------------
+ * TSDFVolume.get_mesh / get_point_cloud of the reference (fusion.py:333-379): marching cubes at level 0 over the
+ * (dims[0],dims[1],dims[2]) C-order tsdf volume, on the device (DESIGN.md 6.6).  A voxel is inside iff its value is < 0
+ * (unobserved voxels hold 255: outside).  mask_dev: (X,Y,Z) uint8 or NULL; voxels whose mask is 0 read as 1.0 (the
+ * volume itself is not written).  Output order does not depend on thread scheduling: vertices by owning grid point in
+ * C order (then +x, +y, +z edge), faces by cell in C order.
+ * Two calls on the same workspace:
+ *   srf_tsdf_mesh_count_host : counts vertices and faces; synchronises the stream (host results, hence _host).
+ *   srf_tsdf_mesh_emit       : writes verts_dev (V,3) float32 world coordinates float32(v*float32(voxel_size) + origin),
+ *                              normals_dev (V,3) float32 unit gradients toward increasing tsdf (0 where the gradient is 0),
+ *                              colors_dev (V,3) uint8 (r,g,b) unfolded from color_dev at the rounded index,
+ *                              faces_dev (F,3) int32 vertex ids; normals / colors / faces may be NULL (not written).
+ * A volume with a dimension < 2 gives an empty mesh; volumes whose counts could overflow int32 are rejected. */
+size_t srf_tsdf_mesh_workspace_bytes(const int* dims);
+int srf_tsdf_mesh_count_host(const float* tsdf_dev, const uint8_t* mask_dev, const int* dims, void* ws, size_t ws_bytes,
+                             long long* n_verts, long long* n_faces, void* stream);
+int srf_tsdf_mesh_emit(const float* tsdf_dev, const float* color_dev, const uint8_t* mask_dev, const int* dims,
+                       const float* origin, double voxel_size, const void* ws, size_t ws_bytes, float* verts_dev,
+                       float* normals_dev, uint8_t* colors_dev, int32_t* faces_dev, void* stream);
+
 /* --- next row: image-side glue of the novel-view sweep (scripts/reconstruction/generate_novel_depths.py:103-152) ---
  * The reference renders an x-major stride-`scale` pixel grid (gw x gh rays, ray = ix*gh + iy), reshapes, transposes
  * and F.interpolate(bilinear)s to (H,W).  srf_upsample_render does that in one pass from the render outputs:

@@ -105,6 +105,11 @@ SYMBOLS = {
                                      C.POINTER(C.c_double), C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                      C.c_int, C.c_double, C.c_float, C.c_void_p]),
     "srf_tsdf_merge": (C.c_int, [C.c_void_p] * 6 + [C.POINTER(C.c_int), C.c_void_p]),
+    "srf_tsdf_mesh_workspace_bytes": (C.c_size_t, [C.POINTER(C.c_int)]),
+    "srf_tsdf_mesh_count_host": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_size_t,
+                                           C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.c_void_p]),
+    "srf_tsdf_mesh_emit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.c_double,
+                                     C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "srf_upsample_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_void_p]),
     "srf_sphere_feature_dims": (None, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

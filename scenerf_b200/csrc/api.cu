@@ -583,6 +583,64 @@ int srf_tsdf_merge(float* tsdf_a, float* weight_a, float* color_a, const float* 
   return check_cuda("srf_tsdf_merge");
 }
 
+namespace {
+// 0 = ok; otherwise the failure already recorded.  *empty = a dimension < 2 (no cell: an empty mesh)
+int mesh_dims(const char* fn, const int* dims, bool* empty) {
+  if (!dims || dims[0] < 1 || dims[1] < 1 || dims[2] < 1)
+    return fail(SRF_E_INVALID, "%s: bad dims", fn);
+  const long long n = (long long)dims[0] * dims[1] * dims[2];
+  // the scanned counts are int32: at most 3 vertices per grid point and 10 faces per cell
+  if (n > 0x7fffffffLL / 10)
+    return fail(SRF_E_INVALID, "%s: volume (%d,%d,%d) too large for int32 vertex / face counts", fn, dims[0], dims[1], dims[2]);
+  *empty = dims[0] < 2 || dims[1] < 2 || dims[2] < 2;
+  return SRF_OK;
+}
+}  // namespace
+
+size_t srf_tsdf_mesh_workspace_bytes(const int* dims) {
+  bool empty;
+  if (mesh_dims("srf_tsdf_mesh_workspace_bytes", dims, &empty)) return 0;
+  return srf::mesh_workspace_bytes(dims);
+}
+
+int srf_tsdf_mesh_count_host(const float* tsdf_dev, const uint8_t* mask_dev, const int* dims, void* ws, size_t ws_bytes,
+                             long long* n_verts, long long* n_faces, void* stream) {
+  bool empty;
+  if (int rc = mesh_dims("srf_tsdf_mesh_count_host", dims, &empty)) return rc;
+  if (!tsdf_dev || !n_verts || !n_faces) return fail(SRF_E_INVALID, "srf_tsdf_mesh_count_host: NULL argument");
+  if (empty) {
+    *n_verts = *n_faces = 0;
+    return SRF_OK;
+  }
+  if (!ws || ws_bytes < srf::mesh_workspace_bytes(dims))
+    return fail(SRF_E_WORKSPACE, "srf_tsdf_mesh_count_host: workspace %zu bytes < %zu", ws_bytes, srf::mesh_workspace_bytes(dims));
+  srf::launch_mesh_count(tsdf_dev, mask_dev, dims, ws, (cudaStream_t)stream);
+  g_launches = 4;
+  if (int rc = check_cuda("srf_tsdf_mesh_count_host")) return rc;
+  int nv = 0, nt = 0;
+  const cudaError_t e = srf::mesh_read_totals(dims, ws, &nv, &nt, (cudaStream_t)stream);
+  if (e != cudaSuccess) return fail(SRF_E_CUDA, "srf_tsdf_mesh_count_host: %s", cudaGetErrorString(e));
+  *n_verts = nv;
+  *n_faces = nt;
+  return SRF_OK;
+}
+
+int srf_tsdf_mesh_emit(const float* tsdf_dev, const float* color_dev, const uint8_t* mask_dev, const int* dims,
+                       const float* origin, double voxel_size, const void* ws, size_t ws_bytes, float* verts_dev,
+                       float* normals_dev, uint8_t* colors_dev, int32_t* faces_dev, void* stream) {
+  bool empty;
+  if (int rc = mesh_dims("srf_tsdf_mesh_emit", dims, &empty)) return rc;
+  if (!tsdf_dev || !origin || !verts_dev || (colors_dev && !color_dev))
+    return fail(SRF_E_INVALID, "srf_tsdf_mesh_emit: NULL argument");
+  if (empty) return SRF_OK;
+  if (!ws || ws_bytes < srf::mesh_workspace_bytes(dims))
+    return fail(SRF_E_WORKSPACE, "srf_tsdf_mesh_emit: workspace %zu bytes < %zu", ws_bytes, srf::mesh_workspace_bytes(dims));
+  srf::launch_mesh_emit(tsdf_dev, color_dev, mask_dev, dims, origin, voxel_size, ws, verts_dev, normals_dev, colors_dev,
+                        faces_dev, (cudaStream_t)stream);
+  g_launches = faces_dev ? 2 : 1;
+  return check_cuda("srf_tsdf_mesh_emit");
+}
+
 int srf_upsample_render(const float* depth_xm, const float* color_xm, int gw, int gh, int out_h, int out_w,
                         float* depth_out, float* color_out, int color_mode, void* stream) {
   if (gw < 1 || gh < 1 || out_h < 1 || out_w < 1 || color_mode < 0 || color_mode > 2)

@@ -23,6 +23,14 @@ void launch_tsdf_integrate(const int* dims, const float* origin, double voxel_si
                            int im_h, int im_w, double trunc, float obs_weight, int color_is_u8, float* tsdf, float* weight,
                            float* color, const float* depth, const void* color_im, cudaStream_t st);
 
+// mesh.cu : marching cubes over a TSDF volume (reference: data/utils/fusion.py:333-379)
+size_t mesh_workspace_bytes(const int* dims);
+void launch_mesh_count(const float* tsdf, const unsigned char* mask, const int* dims, void* ws, cudaStream_t st);
+cudaError_t mesh_read_totals(const int* dims, const void* ws, int* n_verts, int* n_tris, cudaStream_t st);
+void launch_mesh_emit(const float* tsdf, const float* color, const unsigned char* mask, const int* dims, const float* origin,
+                      double voxel_size, const void* ws, float* verts, float* normals, unsigned char* colors, int* faces,
+                      cudaStream_t st);
+
 // image_ops.cu : resampling of x-major renders into images, TSDF volume merge
 void launch_upsample_render(const float* depth_xm, const float* color_xm, int gw, int gh, int H, int W, float* depth_out,
                             float* color_out, int color_mode, cudaStream_t st);

@@ -2,7 +2,9 @@
 (/root/reference/scenerf/data/utils/fusion.py:20-58 constructor, :219-324 integrate, :326-330 get_volume), so that the
 scene-reconstruction script (scripts/reconstruction/depth2tsdf.py:87-103) can consume rendered depth / colour tensors
 straight from device memory instead of the .npy / .png round trip.  Semantics: the reference's CPU (numba) path.
-Marching cubes / mesh export (fusion.py:332-380, skimage) stay with the caller: `get_volume()` returns numpy arrays."""
+`get_mesh` / `get_point_cloud` (fusion.py:333-379, skimage's marching_cubes_lewiner there) run marching cubes on the
+device (csrc/mesh.cu, DESIGN.md 6.6) and return numpy arrays in the reference's order; `get_mesh(mask)` does not
+write into the volume (the reference's CPU path does)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -70,3 +72,42 @@ class TSDFVolume:
 
     def get_weight(self):
         return self._weight.cpu().numpy()
+
+    def _marching_cubes(self, mask, want_faces):
+        """Counts, allocates and emits on the device: (verts, faces or None, normals or None, colors) tensors."""
+        st = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        mask_ptr = None
+        if mask is not None:
+            m = torch.as_tensor(mask)
+            if m.numel() != self._tsdf.numel():
+                raise ValueError("mask has %d elements, the volume %d" % (m.numel(), self._tsdf.numel()))
+            m = m.reshape(-1).to(device=self.device, dtype=torch.bool).to(torch.uint8).contiguous()
+            mask_ptr = m.data_ptr()
+        ws_bytes = self.lib.srf_tsdf_mesh_workspace_bytes(self._dims)
+        ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=self.device)
+        nv, nf = C.c_longlong(0), C.c_longlong(0)
+        _lib.check(self.lib.srf_tsdf_mesh_count_host(self._tsdf.data_ptr(), mask_ptr, self._dims, ws.data_ptr(), ws_bytes,
+                                                     C.byref(nv), C.byref(nf), st))
+        verts = torch.empty((nv.value, 3), dtype=torch.float32, device=self.device)
+        norms = torch.empty((nv.value, 3), dtype=torch.float32, device=self.device) if want_faces else None
+        colors = torch.empty((nv.value, 3), dtype=torch.uint8, device=self.device)
+        faces = torch.empty((nf.value, 3), dtype=torch.int32, device=self.device) if want_faces else None
+        if nv.value:
+            origin = (C.c_float * 3)(*[float(v) for v in self._vol_origin])
+            _lib.check(self.lib.srf_tsdf_mesh_emit(
+                self._tsdf.data_ptr(), self._color.data_ptr(), mask_ptr, self._dims, origin, self._voxel_size, ws.data_ptr(),
+                ws_bytes, verts.data_ptr(), norms.data_ptr() if want_faces else None, colors.data_ptr(),
+                faces.data_ptr() if want_faces else None, st))
+        return verts, faces, norms, colors
+
+    def get_mesh(self, mask=None):
+        """Marching cubes at level 0 (fusion.py:356-379): verts (V,3) float32 world coordinates, faces (F,3) int32,
+        norms (V,3) float32, colors (V,3) uint8.  mask: X*Y*Z booleans (numpy or tensor); voxels where it is False
+        read as 1.0 for this call only."""
+        verts, faces, norms, colors = self._marching_cubes(mask, True)
+        return verts.cpu().numpy(), faces.cpu().numpy(), norms.cpu().numpy(), colors.cpu().numpy()
+
+    def get_point_cloud(self):
+        """The mesh vertices and their colours (fusion.py:333-354)."""
+        verts, _, _, colors = self._marching_cubes(None, False)
+        return verts.cpu().numpy(), colors.cpu().numpy()
