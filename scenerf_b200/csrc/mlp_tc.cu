@@ -32,7 +32,7 @@
 // followed by the image of its low parts and both are accumulated into the same registers:
 //   D[r] = x_hi (W_hi + W_lo)^T ,  D[r+32] = x_lo (W_hi + W_lo)^T ,  result[r] = D[r] + D[r+32]   (epilogue)
 // Row r + 32 sits in the thread 64 above the thread of row r, at the same register index: the epilogue hands those
-// partial sums over through the per-CTA scratch.
+// partial sums over through the warpgroup's (then idle) latent buffer in shared memory, 32 registers per round.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -60,7 +60,7 @@ constexpr int kNumLayers = 11;
 // split-mode blobs: the power-of-two weight scale 2^s and its inverse live in unused entries of the b_out header row
 constexpr int kScaleSlot = 7 * kHidden + 256, kInvScaleSlot = 7 * kHidden + 257;
 // per-CTA scratch (floats): fp32 hidden state (2 warpgroups x 2 quarters x 64 registers x 128 threads), then the
-// split-mode hand-over of the low-part sums (2 x 2 x 64 x 64)
+// split-mode hand-over of the low-part sums of lin_out (the 512-wide layers hand theirs over in shared memory)
 constexpr size_t kScratchFloats = (size_t)2 * kTileM * kHidden;   // 256 KB per CTA
 constexpr size_t kExchangeOffset = (size_t)2 * 2 * 64 * 128;
 
@@ -582,25 +582,31 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     //   h is kept in register order: element (j, i) of thread t at hbuf[(j * 64 + i) * 128 + t]
     auto epilogue = [&](auto use_h_c, auto write_h_c, auto use_p_c, int bias_idx) __attribute__((always_inline)) {
       constexpr bool USE_H = decltype(use_h_c)::value, WRITE_H = decltype(write_h_c)::value, USE_P = decltype(use_p_c)::value;
-      if constexpr (SPLIT) {
-        // low-part sums (rows 32-63, threads 64-127 of the warpgroup) go to the thread 64 below
-        if (t >= 64) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) { xbuf[i * 64 + (t - 64)] = acc0[i]; xbuf[(64 + i) * 64 + (t - 64)] = acc1[i]; }
-        }
-        named_bar_sync(2 + wg, 128);
-        if (t >= 64) return;
-      }
       [[maybe_unused]] const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
+      // split mode: the low-part sums (rows 32-63, threads 64-127 of the warpgroup) go to the thread 64 below through
+      // shared memory, 32 registers per round: the warpgroup's latent buffer (8 KB = 32 registers x 64 threads) is free
+      // in every epilogue -- the MMAs that read it have completed and the next gather comes after the epilogue
+      [[maybe_unused]] float* xs = reinterpret_cast<float*>(smem + kSmemZ + (size_t)wg * kAChunkBytes);   // [reg][hi thread]
       auto finish = [&](float (&acc)[64], int j) __attribute__((always_inline)) {
 #pragma unroll
-        for (int i2 = 0; i2 < 32; ++i2) {
+       for (int half = 0; half < 2; ++half) {
+        if constexpr (SPLIT) {
+          if (j | half) named_bar_sync(2 + wg, 128);               // the previous round has been read
+          if (t >= 64) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) xs[i * 64 + (t - 64)] = acc[32 * half + i];
+          }
+          named_bar_sync(2 + wg, 128);
+          if (t >= 64) continue;
+        }
+#pragma unroll
+        for (int i2 = 16 * half; i2 < 16 * half + 16; ++i2) {
           const int i = 2 * i2, hh = i2 & 1;
           const int row = erow0 + 8 * hh;
           const int col = 256 * wg + 128 * j + 8 * (i2 >> 1) + ecol;
           float r0 = acc[i], r1 = acc[i + 1];
           if constexpr (SPLIT) {
-            const float p0 = xbuf[(j * 64 + i) * 64 + t], p1 = xbuf[(j * 64 + i + 1) * 64 + t];
+            const float p0 = xs[(i - 32 * half) * 64 + t], p1 = xs[(i + 1 - 32 * half) * 64 + t];
             r0 = (r0 + p0) * inv_scale; r1 = (r1 + p1) * inv_scale;      // D_hi + D_lo
           }
           if constexpr (!USE_P) {
@@ -637,6 +643,7 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
             sts32(addr + (uint32_t)row * 128 + inrow, pack_relu_half2(r0, r1));
           }
         }
+       }
       };
       finish(acc0, 0);
       finish(acc1, 1);
