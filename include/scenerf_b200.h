@@ -266,6 +266,39 @@ int srf_tsdf_mesh_emit(const float* tsdf_dev, const float* color_dev, const uint
                        const float* origin, double voxel_size, const void* ws, size_t ws_bytes, float* verts_dev,
                        float* normals_dev, uint8_t* colors_dev, int32_t* faces_dev, void* stream);
 
+/* --- evaluation metrics on the device (DESIGN.md 6.7) ----------------------------------------------------------------
+ * srf_eval_confusion: one pass over a (dims[0],dims[1],dims[2]) C-order volume.  The prediction is either
+ *   - the occupancy of tsdf2occ (eval_sr.py:11-17, eval_sc_bf.py:117-123): pred_dev NULL, tsdf_dev float32, occupied iff
+ *     double(|tsdf|) < th_dev[index along th_axis] and |tsdf| != 255; th_dev holds dims[th_axis] float64 thresholds
+ *     (computed by the caller with the reference's expression and clamps); occ_dev (uint8 0/1) is written if non-NULL;
+ *   - or pred_dev, an array of the srf_eval_dtype pred_dtype (tsdf_dev, th_dev, occ_dev unused).
+ * target_dev: uint8 labels, 255 = not evaluated (NULL in occupancy mode: only occ_dev is written).  mask_dev: uint8 0/1 or NULL.
+ * hist_dev: srf_eval_hist_len(dims, n_classes, per_z) int64 counters, zeroed here and then filled:
+ *   hist[zh][m][tb][pb], zh = z slice (per_z != 0) or 0, m = 0 every voxel / 1 voxels with mask 1,
+ *   tb = target bucket (label l < n_classes -> l, any other label but 255 -> n_classes; 255 is not counted),
+ *   pb = pred bucket (value j in [0, n_classes) -> j, other value > 0 -> n_classes, the rest -> n_classes + 1).
+ *   The tsdf occupancy counts as pred 1 (n_classes + 0 when n_classes == 1).
+ * max_z_dev (one int): the largest z holding a label other than 0 and 255, -1 if none. */
+enum srf_eval_dtype { SRF_EVAL_U8 = 0, SRF_EVAL_I32 = 1, SRF_EVAL_I64 = 2, SRF_EVAL_F32 = 3, SRF_EVAL_F64 = 4 };
+#define SRF_EVAL_MAX_CLASSES 64
+size_t srf_eval_hist_len(const int* dims, int n_classes, int per_z);
+int srf_eval_confusion(const float* tsdf_dev, const void* pred_dev, int pred_dtype, const uint8_t* target_dev,
+                       const uint8_t* mask_dev, const int* dims, int n_classes, int th_axis, const double* th_dev, int per_z,
+                       long long* hist_dev, int* max_z_dev, uint8_t* occ_dev, void* stream);
+/* generate_sc_gt_bf.py:307-309: out_dev = 255, then 0 where tsdf > float32(voxel_size), then 1 where |tsdf| <
+ * float32(voxel_size), both only where tsdf != 255 (float32 comparisons). */
+int srf_eval_sc_label(const float* tsdf_dev, const int* dims, double voxel_size, uint8_t* out_dev, void* stream);
+/* F.interpolate(size=(out_h,out_w), mode="bilinear", align_corners=False) of one row-major float32 image. */
+int srf_resize_bilinear(const float* src_dev, int in_h, int in_w, float* dst_dev, int out_h, int out_w, void* stream);
+/* compute_depth_errors (loss/depth_metrics.py) of n (gt, pred) float32 pairs; pred is clamped to [1e-3, 80] on the fly
+ * (the inputs are not written).  Sums in float64 with a fixed order.  The frame's (abs_rel, sq_rel, rmse, rmse_log,
+ * a1, a2, a3) -- the first four rounded to float32 as the reference returns them -- are written to frame_dev[7] if
+ * non-NULL and added to buckets_dev[slot*8 + 0..6], and buckets_dev[slot*8 + 7] += 1 (frame count), if buckets_dev is
+ * non-NULL.  Nothing synchronises.  ws: srf_depth_errors_workspace_bytes() bytes. */
+size_t srf_depth_errors_workspace_bytes(void);
+int srf_depth_errors(const float* gt_dev, const float* pred_dev, long long n, void* ws, size_t ws_bytes, double* buckets_dev,
+                     int slot, double* frame_dev, void* stream);
+
 /* --- next row: image-side glue of the novel-view sweep (scripts/reconstruction/generate_novel_depths.py:103-152) ---
  * The reference renders an x-major stride-`scale` pixel grid (gw x gh rays, ray = ix*gh + iy), reshapes, transposes
  * and F.interpolate(bilinear)s to (H,W).  srf_upsample_render does that in one pass from the render outputs:

@@ -110,7 +110,15 @@ SYMBOLS = {
                                            C.POINTER(C.c_longlong), C.POINTER(C.c_longlong), C.c_void_p]),
     "srf_tsdf_mesh_emit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float), C.c_double,
                                      C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "srf_upsample_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+    "srf_eval_hist_len": (C.c_size_t, [C.POINTER(C.c_int), C.c_int, C.c_int]),
+    "srf_eval_confusion": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_int,
+                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "srf_eval_sc_label": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_double, C.c_void_p, C.c_void_p]),
+    "srf_resize_bilinear": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "srf_depth_errors_workspace_bytes": (C.c_size_t, []),
+    "srf_depth_errors": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p,
+                                   C.c_void_p]),
+    "srf_upsample_render":(C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_void_p]),
     "srf_sphere_feature_dims": (None, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "srf_sphere_feature": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,

@@ -653,6 +653,67 @@ int srf_upsample_render(const float* depth_xm, const float* color_xm, int gw, in
   return check_cuda("srf_upsample_render");
 }
 
+size_t srf_eval_hist_len(const int* dims, int n_classes, int per_z) {
+  if (!dims || dims[0] < 1 || dims[1] < 1 || dims[2] < 1 || n_classes < 1 || n_classes > SRF_EVAL_MAX_CLASSES) return 0;
+  return srf::eval_hist_len(dims, n_classes, per_z);
+}
+
+int srf_eval_confusion(const float* tsdf_dev, const void* pred_dev, int pred_dtype, const uint8_t* target_dev,
+                       const uint8_t* mask_dev, const int* dims, int n_classes, int th_axis, const double* th_dev, int per_z,
+                       long long* hist_dev, int* max_z_dev, uint8_t* occ_dev, void* stream) {
+  if (!dims || dims[0] < 1 || dims[1] < 1 || dims[2] < 1) return fail(SRF_E_INVALID, "srf_eval_confusion: bad dims");
+  if (n_classes < 1 || n_classes > SRF_EVAL_MAX_CLASSES)
+    return fail(SRF_E_INVALID, "srf_eval_confusion: n_classes=%d outside [1,%d]", n_classes, SRF_EVAL_MAX_CLASSES);
+  if (!hist_dev || !max_z_dev || (!target_dev && (pred_dev || !occ_dev)))
+    return fail(SRF_E_INVALID, "srf_eval_confusion: NULL argument");
+  if (pred_dev) {
+    if (pred_dtype < SRF_EVAL_U8 || pred_dtype > SRF_EVAL_F64)
+      return fail(SRF_E_INVALID, "srf_eval_confusion: unknown pred_dtype %d", pred_dtype);
+  } else {
+    if (!tsdf_dev || !th_dev) return fail(SRF_E_INVALID, "srf_eval_confusion: occupancy mode needs tsdf_dev and th_dev");
+    if (th_axis < 0 || th_axis > 2) return fail(SRF_E_INVALID, "srf_eval_confusion: th_axis=%d outside [0,2]", th_axis);
+  }
+  // one block's histogram lives in shared memory as 32-bit counters
+  const size_t sh = srf::eval_hist_len(dims, n_classes, per_z) * sizeof(unsigned int);
+  if (sh > 200 * 1024)
+    return fail(SRF_E_INVALID, "srf_eval_confusion: %zu histogram bytes per block exceed 200 KB (per_z=%d, n_classes=%d, Z=%d)", sh,
+                per_z, n_classes, dims[2]);
+  srf::launch_eval_confusion(tsdf_dev, pred_dev, pred_dtype, target_dev, mask_dev, dims, n_classes, th_axis, th_dev, per_z,
+                             (unsigned long long*)hist_dev, max_z_dev, occ_dev, (cudaStream_t)stream);
+  g_launches = 1;
+  return check_cuda("srf_eval_confusion");
+}
+
+int srf_eval_sc_label(const float* tsdf_dev, const int* dims, double voxel_size, uint8_t* out_dev, void* stream) {
+  if (!tsdf_dev || !out_dev || !dims || dims[0] < 1 || dims[1] < 1 || dims[2] < 1)
+    return fail(SRF_E_INVALID, "srf_eval_sc_label: bad argument");
+  srf::launch_eval_sc_label(tsdf_dev, (long long)dims[0] * dims[1] * dims[2], (float)voxel_size, out_dev, (cudaStream_t)stream);
+  g_launches = 1;
+  return check_cuda("srf_eval_sc_label");
+}
+
+int srf_resize_bilinear(const float* src_dev, int in_h, int in_w, float* dst_dev, int out_h, int out_w, void* stream) {
+  if (!src_dev || !dst_dev || in_h < 1 || in_w < 1 || out_h < 1 || out_w < 1 || (long long)out_h * out_w > 0x7fffffffLL)
+    return fail(SRF_E_INVALID, "srf_resize_bilinear: bad argument %dx%d -> %dx%d", in_h, in_w, out_h, out_w);
+  srf::launch_resize_bilinear(src_dev, in_h, in_w, dst_dev, out_h, out_w, (cudaStream_t)stream);
+  g_launches = 1;
+  return check_cuda("srf_resize_bilinear");
+}
+
+size_t srf_depth_errors_workspace_bytes(void) { return srf::depth_errors_workspace_bytes(); }
+
+int srf_depth_errors(const float* gt_dev, const float* pred_dev, long long n, void* ws, size_t ws_bytes, double* buckets_dev,
+                     int slot, double* frame_dev, void* stream) {
+  if (!gt_dev || !pred_dev || n < 1) return fail(SRF_E_INVALID, "srf_depth_errors: bad argument (n=%lld)", n);
+  if (!buckets_dev && !frame_dev) return fail(SRF_E_INVALID, "srf_depth_errors: nothing to write (buckets and frame are NULL)");
+  if (buckets_dev && slot < 0) return fail(SRF_E_INVALID, "srf_depth_errors: slot=%d < 0", slot);
+  if (!ws || ws_bytes < srf::depth_errors_workspace_bytes())
+    return fail(SRF_E_WORKSPACE, "srf_depth_errors: workspace %zu bytes < %zu", ws_bytes, srf::depth_errors_workspace_bytes());
+  srf::launch_depth_errors(gt_dev, pred_dev, n, ws, buckets_dev, slot, frame_dev, (cudaStream_t)stream);
+  g_launches = 2;
+  return check_cuda("srf_depth_errors");
+}
+
 int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K, const float* bias,
                    const float* mask, int ldm, const float* residual, int ldr, int accumulate, float* splitk_ws,
                    size_t splitk_ws_floats, int use_tf32, void* stream) {

@@ -12,9 +12,11 @@ namespace srf {
 // (UpSample.h) -> src = scale*(dst+0.5)-0.5 clamped at 0, scale = in/out in float; lambda1 = src - floor, lambda0 = 1-lambda1;
 // value = wy0*(wx0*v00 + wx1*v01) + wy1*(wx0*v10 + wx1*v11).
 struct Tap { int i0, i1; float w0, w1; };
+// FMA: ATen's CPU kernel as compiled (src = fma(scale, dst+0.5, -0.5)); otherwise separately rounded operations
+template <bool FMA = false>
 __device__ __forceinline__ Tap source_tap(int dst, int in_size, int out_size) {
   const float scale = __fdiv_rn((float)in_size, (float)out_size);
-  float src = __fsub_rn(__fmul_rn(scale, __fadd_rn((float)dst, 0.5f)), 0.5f);
+  float src = FMA ? __fmaf_rn(scale, __fadd_rn((float)dst, 0.5f), -0.5f) : __fsub_rn(__fmul_rn(scale, __fadd_rn((float)dst, 0.5f)), 0.5f);
   if (src < 0.f) src = 0.f;
   Tap t;
   t.i0 = min((int)src, in_size - 1);
@@ -81,6 +83,30 @@ __global__ void tsdf_merge_kernel(float* __restrict__ tsdf_a, float* __restrict_
   const float a = tsdf_a[i], b = tsdf_b[i];
   weight_a[i] = weight_a[i] + wb;
   if (!(fabsf(a) < fabsf(b))) { tsdf_a[i] = b; color_a[i] = color_b[i]; }
+}
+
+// One float32 image resized with F.interpolate(size=(out_h, out_w), mode="bilinear", align_corners=False), as
+// generate_sc_gt_bf.py:296-297 resizes each source depth -- a CPU tensor there, so the arithmetic is that of ATen's CPU
+// kernel as built: the source index and each 2-tap lerp contract into one FMA (a*wa + b*wb -> fma(a, wa, b*wb)), outer
+// (y) lerp of the two inner (x) lerps.  The tap indices and weights are those of source_tap, which is the size= form:
+// ATen takes scale = float(in)/out.  The scale_factor= form (recompute_scale_factor unset) takes scale = 1/scale_factor
+// instead, which differs in the last bits whenever in/out is not what 1/scale_factor rounds to.
+__device__ __forceinline__ float lerp_fma(float a, float wa, float b, float wb) { return __fmaf_rn(a, wa, __fmul_rn(b, wb)); }
+
+__global__ void resize_bilinear_kernel(const float* __restrict__ src, int in_h, int in_w, float* __restrict__ dst, int out_h,
+                                       int out_w) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= out_h * out_w) return;
+  const int y = i / out_w, x = i % out_w;
+  const Tap tx = source_tap<true>(x, in_w, out_w), ty = source_tap<true>(y, in_h, out_h);
+  const float* r0 = src + (size_t)ty.i0 * in_w;
+  const float* r1 = src + (size_t)ty.i1 * in_w;
+  dst[i] = lerp_fma(lerp_fma(r0[tx.i0], tx.w0, r0[tx.i1], tx.w1), ty.w0, lerp_fma(r1[tx.i0], tx.w0, r1[tx.i1], tx.w1), ty.w1);
+}
+
+void launch_resize_bilinear(const float* src, int in_h, int in_w, float* dst, int out_h, int out_w, cudaStream_t st) {
+  const int n = out_h * out_w;
+  resize_bilinear_kernel<<<(n + 255) / 256, 256, 0, st>>>(src, in_h, in_w, dst, out_h, out_w);
 }
 
 void launch_upsample_render(const float* depth_xm, const float* color_xm, int gw, int gh, int H, int W, float* depth_out,

@@ -125,6 +125,18 @@ size_t preproj_workspace_bytes(const int* H, const int* W);
 int run_preproject(const DevParams& p, const srf_mlp_weights& w, int fp16, void* table, size_t table_bytes, void* workspace,
                    size_t ws_bytes, cudaStream_t st);
 
+// metrics.cu : evaluation (occupancy confusion histograms, completion-target labels, depth errors)
+size_t eval_hist_len(const int* dims, int n_classes, int per_z);
+void launch_eval_confusion(const float* tsdf, const void* pred, int pred_dtype, const uint8_t* target, const uint8_t* mask,
+                           const int* dims, int n_classes, int th_axis, const double* th, int per_z, unsigned long long* hist,
+                           int* max_z, uint8_t* occ, cudaStream_t st);
+void launch_eval_sc_label(const float* tsdf, long long n, float voxel_size, uint8_t* out, cudaStream_t st);
+size_t depth_errors_workspace_bytes();
+void launch_depth_errors(const float* gt, const float* pred, long long n, void* ws, double* bucket, int slot, double* frame,
+                         cudaStream_t st);
+// image_ops.cu : F.interpolate(size=(out_h,out_w), mode="bilinear", align_corners=False) of one (in_h,in_w) float32 image
+void launch_resize_bilinear(const float* src, int in_h, int in_w, float* dst, int out_h, int out_w, cudaStream_t st);
+
 // non-zero after the kernel's mbarrier watchdog fired: 0x40000000 | warp<<24 | (barrier smem offset)<<4 | parity
 int tc_watchdog_flag();
 // diagnostic: stop every tile after `debug_layer` (1,2,4,5,7,8,9,10 -- see the tile program in mlp_tc.cu) and dump the
