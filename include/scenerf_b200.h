@@ -363,8 +363,10 @@ int srf_debug_tc_layer(const srf_config* cfg, const srf_pyramid* pyr, const srf_
 void srf_set_profiling(int on);
 int srf_last_mlp_ms(float* gauss_ms, float* main_ms);
 
-/* Diagnostic: non-zero once the tensor-core kernel's mbarrier watchdog fired (readable even after the resulting
- * device trap): 0x40000000 | warp << 24 | (barrier smem offset) << 4 | parity. */
+/* Diagnostic: non-zero once the mbarrier watchdog of a TMA-fed tensor-core kernel fired (readable even after the
+ * resulting device trap): 0x40000000 | warp << 24 | (barrier smem offset & 0xFFFFF) << 4 | kernel << 1 | parity, where
+ * kernel is 0 for the point MLP (point_mlp_tc_kernel), 1 for the tf32 GEMM (gemm_tf32_nt_kernel) and 2 for the decoder's
+ * convolution (conv3x3_tf32_kernel). */
 int srf_debug_watchdog_flag(void);
 
 /* Number of kernels the last srf_render_rays / srf_predict call on this thread launched (bench "gpu_launches"). */

@@ -23,7 +23,7 @@ int fail(int code, const char* fmt, ...) {
 
 int check_cuda(const char* what) {
   const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(SRF_E_CUDA, "%s: %s (tc watchdog flag 0x%x)", what, cudaGetErrorString(e), srf::tc_watchdog_flag());
+  if (e != cudaSuccess) return fail(SRF_E_CUDA, "%s: %s (watchdog flag 0x%x)", what, cudaGetErrorString(e), srf::watchdog_flag());
   return SRF_OK;
 }
 
@@ -232,7 +232,7 @@ extern "C" {
 int srf_abi_version(void) { return SRF_ABI_VERSION; }
 const char* srf_last_error(void) { return g_err; }
 int srf_last_launch_count(void) { return g_launches; }
-int srf_debug_watchdog_flag(void) { return srf::tc_watchdog_flag(); }
+int srf_debug_watchdog_flag(void) { return srf::watchdog_flag(); }
 void srf_set_profiling(int on) { g_profiling = on != 0; }
 int srf_last_mlp_ms(float* gauss_ms, float* main_ms) {
   float* dst[2] = {gauss_ms, main_ms};
@@ -725,9 +725,7 @@ int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, i
   const int rc = use_tf32 ? srf::launch_gemm_tf32(g, (cudaStream_t)stream) : srf::launch_gemm(g, (cudaStream_t)stream);
   if (rc) return fail(SRF_E_INVALID, "srf_debug_gemm: shape not supported by the %s kernel", use_tf32 ? "tf32" : "simt");
   g_launches = 1;
-  const int e = check_cuda("srf_debug_gemm");
-  if (e && use_tf32) return fail(SRF_E_CUDA, "srf_debug_gemm: %s (tf32 watchdog flag 0x%x)", srf_last_error(), srf::tf32_watchdog_flag());
-  return e;
+  return check_cuda("srf_debug_gemm");
 }
 
 static int py_round_div(int a, int b) {            // Python round(a / b): half to even
@@ -782,9 +780,7 @@ int srf_conv3x3_hwc(const float* in_dev, int H, int W, int ld_in, const float* w
   if (rc) return fail(SRF_E_INVALID, "srf_conv3x3_hwc: shape or alignment not supported (H=%d W=%d ld_in=%d Cout=%d dil=%d; strides must be "
                                      "multiples of 4 floats, pointers 16-byte aligned)", H, W, ld_in, Cout, dil);
   g_launches = 1;
-  const int e = check_cuda("srf_conv3x3_hwc");
-  if (e) return fail(SRF_E_CUDA, "%s (conv watchdog flag 0x%x)", srf_last_error(), srf::conv_watchdog_flag());
-  return e;
+  return check_cuda("srf_conv3x3_hwc");
 }
 
 int srf_debug_tc_layer(const srf_config* cfg, const srf_pyramid* pyr, const srf_mlp_weights* w,

@@ -10,8 +10,8 @@
 //   in shared memory as the same 128-row x 128-byte swizzled tile a plain GEMM would stage.
 //   B tiles: 2-D map over the weights repacked [tap][co][ci] (ci padded to a multiple of 4), box {32, 128} at (c0, tap*Cout + n0).
 //   wgmma .tf32 (fp32 operands read in place, 10-bit mantissa -- the regime of the reference's own cuDNN default
-//   `allow_tf32=True` on Ampere-class GPUs), 3-stage mbarrier ring fed by one TMA thread, two consumer warpgroups that each
-//   accumulate 64 pixels x 128 channels in registers (wgmma m64n128k8).
+//   `allow_tf32=True` on Ampere-class GPUs) through the tf32 tile mainloop of tma.cuh: two consumer warpgroups that each
+//   accumulate 64 pixels x 128 channels in registers.
 //   The tensor core TRUNCATES the 13 low mantissa bits of what it reads; through the decoder's 35 chained convolutions that
 //   bias compounds (1.3 % relative L2 on the finest map of the test network).  So every tensor that feeds a convolution is
 //   stored already ROUNDED TO NEAREST tf32 (weights at pack time, the concat buffer, intermediate activations: `round_out`),
@@ -20,49 +20,14 @@
 //   (+ residual[p, co]), LeakyReLU, store fp32 [H][W][C] and/or fp16 [H][W][C] -- i.e. straight into the packed pyramid
 //   layout of srf_pyramid (no CHW -> HWC pass).
 // Roofline: tensor (tf32 = half the f16 rate); 2*9*Cin*Cout flops per pixel.
-#include <cuda.h>
 #include <cuda_fp16.h>
 #include "kernels.cuh"
-#include "wgmma.cuh"
+#include "tma.cuh"
 
 namespace srf {
 namespace conv {
 
-constexpr int kBM = 128, kBN = 128, kBK = 32, kStages = 3;
-constexpr uint32_t kTileBytes = kBM * kBK * 4;            // 16 KB
-constexpr int kThreads = 384;                             // warpgroup 0: TMA producer (one thread); 1, 2: MMA + epilogue
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* err) {     // bounded: a protocol bug must not hang the GPU
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 2000000000LL) { if (err) atomicExch(err, (int)(0x43000000u | (bar & 0xFFFFFF))); __trap(); }
-  }
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
+using namespace tf32;
 
 struct ConvArgs {
   int H, W, Cin, Cout;            // Cin as stored (channel stride of the input, multiple of 4; padded channels hold zeros)
@@ -83,59 +48,21 @@ __device__ __forceinline__ float round_tf32(float x) { return __uint_as_float((_
 
 __global__ void __launch_bounds__(kThreads, 1)
 conv3x3_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvArgs a) {
-  extern __shared__ unsigned char smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;            // SWIZZLE_128B tiles need 1024-byte alignment
-  const uint32_t sA = base, sB = base + kStages * kTileBytes;
-  const uint32_t bars = sB + kStages * kTileBytes;                        // full[kStages], empty[kStages]
-  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int xt = (a.W + kBM - 1) / kBM;
   const int y = blockIdx.y / xt, x0 = (blockIdx.y % xt) * kBM;
   const int n0 = blockIdx.x * kBN;
   const int kb = (a.Cin + kBK - 1) / kBK;                                 // channel blocks per tap
-  const int nk = 9 * kb;
-
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    for (int s = 0; s < kStages; ++s) { mbar_init(bars + 8u * s, 1); mbar_init(bars + 8u * (kStages + s), 2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    if (t == 0) {
-      for (int j = 0; j < nk; ++j) {
+  int j = 0;                                                              // the producer's k-block cursor
+  float acc[64];
+  if (!mainloop<kWatchConvTf32>(&tmA, &tmB, 9 * kb, a.err, acc, [&](uint32_t sA, uint32_t sB, uint32_t bar) {
         const int tap = j / kb, cb = j - tap * kb;
         const int dy = (tap / 3 - 1) * a.dil, dx = (tap % 3 - 1) * a.dil;
-        const int s = j % kStages;
-        mbar_wait(bars + 8u * (kStages + s), (((uint32_t)(j / kStages)) & 1u) ^ 1u, a.err);
-        mbar_arrive_expect_tx(bars + 8u * s, 2 * kTileBytes);
-        tma_load_3d(sA + s * kTileBytes, &tmA, cb * kBK, x0 + dx, y + dy, bars + 8u * s);      // OOB -> zeros = the conv padding
-        tma_load_2d(sB + s * kTileBytes, &tmB, cb * kBK, tap * a.Cout + n0, bars + 8u * s);
-      }
-    }
+        tma_load_3d(sA, &tmA, cb * kBK, x0 + dx, y + dy, bar);      // OOB -> zeros = the conv padding
+        tma_load_2d(sB, &tmB, cb * kBK, tap * a.Cout + n0, bar);
+        ++j;
+      }))
     return;
-  }
-  // consumer warpgroup: pixels x0 + (wg - 1) * 64 .. +63 (the A tile's 64-row half starts 8 KB further)
-  const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  for (int j = 0; j < nk; ++j) {
-    const int s = j % kStages;
-    mbar_wait(bars + 8u * s, ((uint32_t)(j / kStages)) & 1u, a.err);
-    gmma::fence();
-#pragma unroll
-    for (int k4 = 0; k4 < kBK / 8; ++k4)
-      gmma::mma_tf32_n128(acc, gmma::desc_sw128(sA + s * kTileBytes + a_off + k4 * 32), gmma::desc_sw128(sB + s * kTileBytes + k4 * 32),
-                          (j > 0 || k4 > 0) ? 1 : 0);
-    gmma::commit();
-    // this stage's MMAs stay in flight; the previous stage has completed and goes back to the producer
-    gmma::wait<1>();
-    if (t == 0 && j > 0) mbar_arrive(bars + 8u * (kStages + (j - 1) % kStages));
-  }
-  gmma::wait<0>();
-  gmma::fence_regs(acc);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
   const int w = t >> 5, l = t & 31;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
@@ -193,67 +120,28 @@ __global__ void upsample_concat_kernel(const float* __restrict__ x, int h, int w
 
 }  // namespace conv
 
-using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn conv_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
-static int* g_conv_err = nullptr;
-int conv_watchdog_flag() { return g_conv_err ? *reinterpret_cast<volatile int*>(g_conv_err) : 0; }
-
 // in: [H][W][Cin] float32 (Cin = channel stride, multiple of 4, 16-byte aligned); w9: [9][Cout][Cin] float32 (tap = ky*3 + kx).
 // Returns 0, -1 (shape / alignment not expressible as tensor maps), -2 (driver entry point missing).
 int launch_conv3x3_tf32(const float* in, int H, int W, int Cin, const float* w9, int Cout, int dil, const float* scale, const float* shift,
                         const float* residual, int ld_res, float slope, int round_out, float* out32, int ld32, void* out16, int ld16,
                         cudaStream_t st) {
-  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (H < 1 || W < 1 || Cin < 4 || (Cin % 4) || Cout < 4 || (Cout % 4) || dil < 1 || !al16(in) || !al16(w9) || !al16(scale) || !al16(shift)) return -1;
   if ((out32 && (!al16(out32) || ld32 % 4)) || (out16 && ((reinterpret_cast<uintptr_t>(out16) & 7) || ld16 % 4)) || (residual && (!al16(residual) || ld_res % 4)))
     return -1;
-  EncodeTiledFn fn = conv_encode_fn();
-  if (!fn) return -2;
   CUtensorMap tmA, tmB;
-  {
-    const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H};
-    const cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)W * Cin * 4};
-    const cuuint32_t box[3] = {(cuuint32_t)conv::kBK, (cuuint32_t)conv::kBM, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    if (fn(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return -1;
-  }
-  {
-    const cuuint64_t dims[2] = {(cuuint64_t)Cin, (cuuint64_t)9 * Cout};
-    const cuuint64_t strides[1] = {(cuuint64_t)Cin * 4};
-    const cuuint32_t box[2] = {(cuuint32_t)conv::kBK, (cuuint32_t)conv::kBN};
-    const cuuint32_t estr[2] = {1, 1};
-    if (fn(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w9), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return -1;
-  }
-  if (!g_conv_err) {
-    int* h = nullptr;
-    if (cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped) == cudaSuccess) { *h = 0; cudaHostGetDevicePointer(&g_conv_err, h, 0); }
-  }
+  const cuuint64_t dims_a[3] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H}, strides_a[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)W * Cin * 4};
+  const cuuint64_t dims_b[2] = {(cuuint64_t)Cin, (cuuint64_t)9 * Cout}, strides_b[1] = {(cuuint64_t)Cin * 4};
+  const cuuint32_t box_a[3] = {(cuuint32_t)tf32::kBK, (cuuint32_t)tf32::kBM, 1}, box_b[2] = {(cuuint32_t)tf32::kBK, (cuuint32_t)tf32::kBN};
+  int rc = encode_tensor_map_f32(&tmA, in, 3, dims_a, strides_a, box_a);
+  if (rc == 0) rc = encode_tensor_map_f32(&tmB, w9, 2, dims_b, strides_b, box_b);
+  if (rc) return rc;
   static bool attr = false;
-  const size_t smem = 2 * conv::kStages * conv::kTileBytes + 1024 + 64;
-  if (!attr) { cudaFuncSetAttribute(conv::conv3x3_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+  if (!attr) { cudaFuncSetAttribute(conv::conv3x3_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tf32::kSmemBytes); attr = true; }
   conv::ConvArgs a;
   a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.dil = dil; a.scale = scale; a.shift = shift; a.residual = residual; a.ld_res = ld_res;
-  a.slope = slope; a.round_out = round_out; a.out32 = out32; a.ld32 = ld32; a.out16 = reinterpret_cast<__half*>(out16); a.ld16 = ld16; a.err = g_conv_err;
-  const dim3 grid((Cout + conv::kBN - 1) / conv::kBN, (unsigned)(H * ((W + conv::kBM - 1) / conv::kBM)));
-  conv::conv3x3_tf32_kernel<<<grid, conv::kThreads, smem, st>>>(tmA, tmB, a);
+  a.slope = slope; a.round_out = round_out; a.out32 = out32; a.ld32 = ld32; a.out16 = reinterpret_cast<__half*>(out16); a.ld16 = ld16; a.err = watchdog_device_flag();
+  const dim3 grid((Cout + tf32::kBN - 1) / tf32::kBN, (unsigned)(H * ((W + tf32::kBM - 1) / tf32::kBM)));
+  conv::conv3x3_tf32_kernel<<<grid, tf32::kThreads, tf32::kSmemBytes, st>>>(tmA, tmB, a);
   return 0;
 }
 

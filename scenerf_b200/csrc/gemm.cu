@@ -192,15 +192,36 @@ gemm128_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B
 // C[m][n] = (accumulate ? C[m][n] : 0) + sum_z part[z][m][n]   (z ascending: deterministic)
 __global__ void __launch_bounds__(256)
 splitk_reduce_kernel(const float* __restrict__ part, int splits, float* __restrict__ C, int ldc, int M, int N, int accumulate,
-                     const int* __restrict__ skip) {
+                     const int* __restrict__ skip, const __grid_constant__ SegInfo sg) {
   if (skip && *skip == 0) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M * N) return;
+  if (sg.mode == 2) {                                      // columns of a dead tile were never written by the GEMM
+    const int t0 = (i % N) / kSegTileN * kSegTileN;
+    if (seg_dead(sg, t0, min(N, t0 + kSegTileN))) return;
+  }
   const int m = i / N, n = i % N;
   float v = 0.f;
   for (int z = 0; z < splits; ++z) v += part[(size_t)z * M * N + i];
   float* dst = C + (size_t)m * ldc + n;
   *dst = accumulate ? (*dst + v) : v;
+}
+
+void launch_splitk_reduce(const GemmArgs& g, int splits, const SegInfo& sg, cudaStream_t st) {
+  splitk_reduce_kernel<<<(g.M * g.N + 255) / 256, 256, 0, st>>>(g.splitk_ws, splits, g.C, g.ldc, g.M, g.N, g.accumulate, g.skip_if_zero, sg);
+}
+
+SplitK plan_splitk(const GemmArgs& g, int tiles, int k_gran, int cap) {
+  SplitK sk{1, g.K};
+  if (!g.splitk_ws || g.bias || g.mask || g.R || tiles >= 96 || g.K < 1024) return sk;
+  int splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
+  if (splits > cap) splits = cap;
+  while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
+  if (splits > 1) {
+    sk.k_per = ((g.K + splits - 1) / splits + k_gran - 1) / k_gran * k_gran;
+    sk.splits = (g.K + sk.k_per - 1) / sk.k_per;             // still >= 2: k_per < K for K >= 1024, k_gran <= 32
+  }
+  return sk;
 }
 
 int device_sm_count() {
@@ -221,8 +242,6 @@ int& launch_counter() {
   return c;
 }
 
-static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 template <bool AT, bool BT, bool RA, bool RB>
 static void dispatch(const GemmArgs& g, cudaStream_t st) {
   bool fast = (g.lda % 4 == 0) && (g.ldb % 4 == 0) && (g.ldc % 4 == 0) && (g.N % 4 == 0) && al16(g.A) && al16(g.B) && al16(g.C);
@@ -233,23 +252,17 @@ static void dispatch(const GemmArgs& g, cudaStream_t st) {
   if (g.mask) fast = fast && al16(g.mask) && (g.ldm % 4 == 0);
   if (g.R) fast = fast && al16(g.R) && (g.ldr % 4 == 0);
   fast = fast && g.M >= 64 && g.N >= 64;
+  // the SIMT kernels write every column: segment mode 0 for the reduce, whatever a tf32-mode fallback call carries in seg_*
+  const SegInfo no_seg{};
   if (fast) {
     dim3 grid((g.N + kBN - 1) / kBN, (g.M + kBM - 1) / kBM);
     // weight-gradient shapes (few output tiles, long K): split K over gridDim.z into the caller's scratch
-    const int tiles = grid.x * grid.y;
-    int splits = 1;
-    if (g.splitk_ws && !g.bias && !g.mask && !g.R && tiles < 96 && g.K >= 1024) {
-      splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
-      if (splits > 16) splits = 16;
-      while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
-    }
-    if (splits > 1) {
-      int k_per = ((g.K + splits - 1) / splits + kBK - 1) / kBK * kBK;
-      splits = (g.K + k_per - 1) / k_per;
-      grid.z = splits;
+    const SplitK sk = plan_splitk(g, grid.x * grid.y, kBK, 16);
+    if (sk.splits > 1) {
+      grid.z = sk.splits;
       gemm128_kernel<AT, BT, RA, RB><<<grid, 256, 0, st>>>(g.A, g.lda, g.B, g.ldb, g.splitk_ws, g.N, g.M, g.N, g.K, nullptr, nullptr, 0,
-                                                           nullptr, 0, 0, k_per, g.skip_if_zero);
-      splitk_reduce_kernel<<<(g.M * g.N + 255) / 256, 256, 0, st>>>(g.splitk_ws, splits, g.C, g.ldc, g.M, g.N, g.accumulate, g.skip_if_zero);
+                                                           nullptr, 0, 0, sk.k_per, g.skip_if_zero);
+      launch_splitk_reduce(g, sk.splits, no_seg, st);
       launch_counter() += 2;
     } else {
       ++launch_counter();
@@ -258,20 +271,12 @@ static void dispatch(const GemmArgs& g, cudaStream_t st) {
     }
   } else {
     dim3 grid((g.N + 63) / 64, (g.M + 63) / 64);
-    const int tiles = grid.x * grid.y;
-    int splits = 1;
-    if (g.splitk_ws && !g.bias && !g.mask && !g.R && tiles < 96 && g.K >= 1024) {
-      splits = (2 * device_sm_count() + tiles - 1) / tiles;     // ~2 waves
-      if (splits > 64) splits = 64;
-      while (splits > 1 && (size_t)splits * g.M * g.N > g.splitk_ws_floats) --splits;
-    }
-    if (splits > 1) {
-      int k_per = ((g.K + splits - 1) / splits + 15) / 16 * 16;
-      splits = (g.K + k_per - 1) / k_per;
-      grid.z = splits;
+    const SplitK sk = plan_splitk(g, grid.x * grid.y, 16, 64);
+    if (sk.splits > 1) {
+      grid.z = sk.splits;
       gemm64_kernel<AT, BT, RA, RB><<<grid, 256, 0, st>>>(g.A, g.lda, g.B, g.ldb, g.splitk_ws, g.N, g.M, g.N, g.K, nullptr, nullptr, 0,
-                                                          nullptr, 0, 0, k_per, g.skip_if_zero);
-      splitk_reduce_kernel<<<(g.M * g.N + 255) / 256, 256, 0, st>>>(g.splitk_ws, splits, g.C, g.ldc, g.M, g.N, g.accumulate, g.skip_if_zero);
+                                                          nullptr, 0, 0, sk.k_per, g.skip_if_zero);
+      launch_splitk_reduce(g, sk.splits, no_seg, st);
       launch_counter() += 2;
     } else {
       ++launch_counter();

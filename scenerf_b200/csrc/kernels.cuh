@@ -48,6 +48,14 @@ int run_point_mlp_simt(const DevParams& p, const srf_mlp_weights& w, const float
 void launch_sphere_feature(const float* x, int C, int h, int w, const float* pix, const long long* pix_sphere, int n, int scale,
                            int oW, int oH, int* winner, float* out, int out_hwc, cudaStream_t st);
 
+inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Mapped host flag of the mbarrier watchdog of the sm_90a kernels (tma.cuh), readable even after the resulting device
+// trap: 0, or 0x40000000 | warp << 24 | (barrier smem offset & 0xFFFFF) << 4 | kernel << 1 | parity, where kernel is
+// 0 for point_mlp_tc_kernel, 1 for gemm_tf32_nt_kernel and 2 for conv3x3_tf32_kernel.
+int watchdog_flag();
+int* watchdog_device_flag();   // the device address the kernels write (allocated on first use; null if that failed)
+
 // gemm.cu : float32 SIMT GEMM (see the file header for operand layouts and the epilogue)
 struct GemmArgs {
   const float* A = nullptr; int lda = 0; bool at = false; bool relu_a = false;
@@ -63,6 +71,24 @@ struct GemmArgs {
   float* relu_out = nullptr; int ld_relu = 0;   // tf32 kernel only: the epilogue also stores max(result, 0) here (the next GEMM's A operand)
 };
 int launch_gemm(const GemmArgs& g, cudaStream_t st);
+// The seg_* fields as the tf32 kernel and the split-K reduce read them: mode 0 none, 1 dead k-blocks, 2 dead column tiles
+// of kSegTileN (the tf32 kernel's N tile).
+constexpr int kSegTileN = 128;
+struct SegInfo { const int* flags; int mode; int off[6]; };
+// true when [lo, hi) of the latent axis touches only scales whose flag is 0
+__device__ __forceinline__ bool seg_dead(const SegInfo& sg, int lo, int hi) {
+#pragma unroll
+  for (int s = 0; s < 5; ++s)
+    if (lo < sg.off[s + 1] && hi > sg.off[s] && sg.flags[s] != 0) return false;
+  return true;
+}
+// Deterministic split-K of the weight-gradient shapes (few output tiles, long K): slice z of K (k_per long, a multiple of
+// the kernel's k granularity) goes to g.splitk_ws + z*M*N, then launch_splitk_reduce adds the slices in z order into C.
+// Only for plain products (no bias / mask / residual) of fewer than 96 tiles with K >= 1024: about two waves over the
+// SMs, at most `cap` slices, as many as fit g.splitk_ws_floats.  splits == 1: no split (k_per = K).
+struct SplitK { int splits, k_per; };
+SplitK plan_splitk(const GemmArgs& g, int tiles, int k_gran, int cap);
+void launch_splitk_reduce(const GemmArgs& g, int splits, const SegInfo& sg, cudaStream_t st);
 // SM count of the current device (cached; 132 on an H100 SXM): sizes waves, split-K factors and point chunks
 int device_sm_count();
 // per-thread count of kernels launched by the float32 / tf32 MLP paths (gemm.cu, gemm_tf32.cu, mlp_simt.cu, backward.cu);
@@ -72,7 +98,6 @@ int& launch_counter();    // 0, or -1 for an operand-layout combination that is 
 // gemm_tf32.cu : the same contract on tensor cores (wgmma .tf32, float32 operands read in place); NT layout only
 // (at=false, bt=true, no operand ReLU).  Returns 0, or -1 when the shape cannot be expressed as TMA tensor maps.
 int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st);
-int tf32_watchdog_flag();
 
 // one warp per point: X[i] = [ gathered latent (d_latent) | positional encoding (39) | viewdir (3) | 0-pad ], row stride ld
 //   scale_any (5 ints, or NULL): set to 1 for every scale at which some point of the chunk has an in-range bilinear tap.
@@ -116,7 +141,6 @@ int launch_conv3x3_tf32(const float* in, int H, int W, int Cin, const float* w9,
                         cudaStream_t st);
 void launch_upsample_concat(const float* x, int h, int w, int Cx, int ldx, const float* skip, int Cs, int lds, int H, int W, float* out, int ld,
                             cudaStream_t st);
-int conv_watchdog_flag();
 
 // preproj.cu : pre-projected latent table  table[(sy,sx)][block][512] = lin_z[block].weight . z(sphere pixel)  (see file header)
 size_t preproj_rows(int sphere_W, int sphere_H);
@@ -137,8 +161,6 @@ void launch_depth_errors(const float* gt, const float* pred, long long n, void* 
 // image_ops.cu : F.interpolate(size=(out_h,out_w), mode="bilinear", align_corners=False) of one (in_h,in_w) float32 image
 void launch_resize_bilinear(const float* src, int in_h, int in_w, float* dst, int out_h, int out_w, cudaStream_t st);
 
-// non-zero after the kernel's mbarrier watchdog fired: 0x40000000 | warp<<24 | (barrier smem offset)<<4 | parity
-int tc_watchdog_flag();
 // diagnostic: stop every tile after `debug_layer` (1,2,4,5,7,8,9,10 -- see the tile program in mlp_tc.cu) and dump the
 // raw fp32 accumulator (n_tiles*64, 512) to debug_acc
 int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n,

@@ -40,7 +40,7 @@
 #include <cstring>
 #include <type_traits>
 #include "kernels.cuh"
-#include "wgmma.cuh"
+#include "tma.cuh"
 
 namespace srf {
 namespace tc {
@@ -107,42 +107,6 @@ struct KernelArgs {
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must not hang the GPU -- after ~2 s the watchdog records the barrier and traps.
-__device__ __noinline__ void mbar_timeout(int* error_flag, uint32_t bar, uint32_t parity) {
-  if (error_flag) atomicExch(error_flag, (int)(0x40000000u | ((bar & 0xFFFFF) << 4) | (parity & 1) | ((threadIdx.x >> 5) << 24)));
-  __threadfence_system();
-  __trap();
-}
-__device__ __noinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity, int* error_flag) {
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) mbar_timeout(error_flag, bar, parity);
-  }
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* error_flag) {
-  if (mbar_try_wait(bar, parity)) return;
-  mbar_wait_spin(bar, parity, error_flag);
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // The 2 x 10.9 MB of weight images are re-read by every CTA for every tile while the feature pyramid streams through
@@ -299,7 +263,7 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
   // wait for the next slot and issue its MMAs: A chunk at a_addr, 4 k-steps of 16 (x hi/lo images)
   auto wait_slot = [&]() -> uint32_t {
     const int s = (int)(cpos % kSlots);
-    mbar_wait(full_bar(s), (cpos / kSlots) & 1u, a.error_flag);
+    mbar_wait<kWatchPointMlp>(full_bar(s), (cpos / kSlots) & 1u, a.error_flag);
     return ring + (uint32_t)s * kSlotBytes;
   };
   // all but the newest commit group have completed: their slots are refilled
@@ -884,10 +848,6 @@ int pack_weights_tc(const srf_mlp_weights& w, void* dst, size_t bytes, int split
   return 0;
 }
 
-static int* g_wd_host = nullptr;
-static int* g_wd_dev = nullptr;
-int tc_watchdog_flag() { return g_wd_host ? *g_wd_host : 0; }
-
 static int num_sms() { return device_sm_count(); }
 
 using TcKernelFn = void (*)(const DevParams, const tc::KernelArgs);
@@ -940,14 +900,7 @@ int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const f
     a.skip_zero = 0;
   }
   a.debug_layer = debug_layer; a.debug_acc = debug_acc;
-  // watchdog flag in mapped pinned host memory: still readable after a device-side trap killed the context
-  if (!g_wd_host) {
-    if (cudaHostAlloc(reinterpret_cast<void**>(&g_wd_host), sizeof(int), cudaHostAllocMapped) == cudaSuccess) {
-      *g_wd_host = 0;
-      cudaHostGetDevicePointer(reinterpret_cast<void**>(&g_wd_dev), g_wd_host, 0);
-    }
-  }
-  a.error_flag = g_wd_dev;
+  a.error_flag = watchdog_device_flag();
   // persistent: one CTA per SM (the shared-memory footprint allows no second one), tiles round-robin
   int grid = a.n_tiles < num_sms() ? a.n_tiles : num_sms();
   if (grid > kMaxTcCtas) grid = kMaxTcCtas;
