@@ -138,8 +138,9 @@ srf::DevParams make_params(const srf_config* cfg, const srf_pyramid* pyr) {
   return p;
 }
 
-size_t mlp_workspace_bytes(int precision, int d_latent, int n_points) {
-  return precision == SRF_PREC_FP32 ? srf::simt_workspace_bytes(d_latent, n_points)
+// save_activations: the float32 pass is a training forward (SRF_FLAG_SAVE_ACTIVATIONS)
+size_t mlp_workspace_bytes(int precision, int d_latent, int n_points, bool save_activations) {
+  return precision == SRF_PREC_FP32 ? srf::simt_workspace_bytes(d_latent, n_points, save_activations)
                                     : srf::tc_workspace_bytes(d_latent, n_points);
 }
 
@@ -161,10 +162,11 @@ int run_mlp(const srf::DevParams& p, int precision, int flags, const srf_mlp_wei
   int l;
   const int pass = (w.d_out == 4) ? 1 : 0;
   prof_record(2 * pass, st);
-  if (precision == SRF_PREC_FP32 && saved)
-    l = srf::run_point_mlp_forward_save(p, w, pts, viewdir, n, n_per, raw, dbg, saved, (flags & SRF_FLAG_TF32_MATMUL) ? 1 : 0, ws, ws_bytes, st);
-  else if (precision == SRF_PREC_FP32) l = srf::run_point_mlp_simt(p, w, pts, viewdir, n, n_per, raw, dbg, ws, ws_bytes, st);
-  else {
+  if (precision == SRF_PREC_FP32) {
+    // SRF_FLAG_TF32_MATMUL applies to the training forward only
+    const srf::MatmulEngine e = (saved && (flags & SRF_FLAG_TF32_MATMUL)) ? srf::MatmulEngine::tf32 : srf::MatmulEngine::simt;
+    l = srf::run_point_mlp_simt(p, w, pts, viewdir, n, n_per, raw, dbg, saved, e, ws, ws_bytes, st);
+  } else {
     int f = flags & ~(srf::kTcFlagSplit | srf::kTcFlagPreproj);
     if (precision == SRF_PREC_FP32_TC) f |= srf::kTcFlagSplit;
     // a latent table belongs to one network: the main pass (d_out 4) reads latent_table, the proposal pass latent_table_gauss
@@ -206,16 +208,13 @@ size_t carve(const srf_config* cfg, int R, int d_latent, unsigned char* base, Ra
   w.depth_volume = a.take<float>((size_t)R * S);
   w.pts = a.take<float>((size_t)R * S * 3);
   w.raw = a.take<float>((size_t)R * S * 4);
-  size_t m1 = mlp_workspace_bytes(cfg->precision, d_latent, (int)((size_t)R * S));
-  const size_t m2 = mlp_workspace_bytes(cfg->precision, d_latent, (int)((size_t)R * G));
-  if ((cfg->flags & SRF_FLAG_SAVE_ACTIVATIONS) && cfg->precision == SRF_PREC_FP32) {       // the training forward's own scratch
-    const size_t m3 = srf::mlp_forward_save_scratch_bytes((int)((size_t)R * S));
-    if (m3 > m1) m1 = m3;
-  }
+  const bool save = (cfg->flags & SRF_FLAG_SAVE_ACTIVATIONS) && cfg->precision == SRF_PREC_FP32;
+  const size_t m1 = mlp_workspace_bytes(cfg->precision, d_latent, (int)((size_t)R * S), save);
+  const size_t m2 = mlp_workspace_bytes(cfg->precision, d_latent, (int)((size_t)R * G), save);
   w.mlp_ws_bytes = m1 > m2 ? m1 : m2;
   w.mlp_ws = a.take<unsigned char>(w.mlp_ws_bytes);
   w.saved_main = w.saved_gauss = nullptr;
-  if ((cfg->flags & SRF_FLAG_SAVE_ACTIVATIONS) && cfg->precision == SRF_PREC_FP32) {
+  if (save) {
     w.saved_main = a.take<unsigned char>(srf::mlp_saved_bytes(d_latent, (int)((size_t)R * S)));
     w.saved_gauss = a.take<unsigned char>(srf::mlp_saved_bytes(d_latent, (int)((size_t)R * G)));
   }
@@ -429,7 +428,7 @@ int srf_render_rays_host(const srf_config* cfg, const srf_pyramid* pyr, const sr
 
 size_t srf_predict_workspace_bytes(const srf_config* cfg, int n_points) {
   if (!cfg || n_points < 0) return 0;
-  return mlp_workspace_bytes(cfg->precision, cfg->d_latent > 0 ? cfg->d_latent : kDefaultLatent, n_points) + align256((size_t)n_points * 4 * 4) + 4096;
+  return mlp_workspace_bytes(cfg->precision, cfg->d_latent > 0 ? cfg->d_latent : kDefaultLatent, n_points, false) + align256((size_t)n_points * 4 * 4) + 4096;
 }
 
 __global__ void activate_kernel(const float* __restrict__ raw, int n, float* __restrict__ density,
@@ -465,7 +464,7 @@ int srf_predict(const srf_config* cfg, const srf_pyramid* pyr, const srf_mlp_wei
   const int n = n_cols * n_per;
   Arena a{reinterpret_cast<unsigned char*>(workspace_dev), 0, 0};
   float* raw = raw_out_dev ? raw_out_dev : a.take<float>((size_t)n * 4);
-  const size_t mlp_bytes = mlp_workspace_bytes(cfg->precision, d_latent, n);
+  const size_t mlp_bytes = mlp_workspace_bytes(cfg->precision, d_latent, n, false);
   if (!workspace_dev || workspace_bytes < a.off + mlp_bytes)
     return fail(SRF_E_WORKSPACE, "srf_predict: workspace has %zu bytes, need %zu", workspace_bytes, a.off + mlp_bytes);
   const srf::DevParams p = make_params(cfg, pyr);
@@ -531,8 +530,8 @@ int srf_render_rays_backward(const srf_config* cfg, const srf_pyramid* pyr, cons
   float* graw_gauss = a.take<float>((size_t)R * G * 2);
   const size_t mlp_ws_bytes = workspace_bytes - a.off - 2048;
   void* mlp_ws = a.take<unsigned char>(mlp_ws_bytes);
-  const int tf32 = (cfg->flags & SRF_FLAG_TF32_MATMUL) ? 1 : 0;
-  if (tf32 && !fw.saved_main)
+  const srf::MatmulEngine e = (cfg->flags & SRF_FLAG_TF32_MATMUL) ? srf::MatmulEngine::tf32 : srf::MatmulEngine::simt;
+  if (e == srf::MatmulEngine::tf32 && !fw.saved_main)
     return fail(SRF_E_INVALID, "srf_render_rays_backward: SRF_FLAG_TF32_MATMUL needs SRF_FLAG_SAVE_ACTIVATIONS (forward and backward must "
                                "see the same activations)");
   srf::launch_ray_backward(p, R, fw.raw, fw.t_sorted, fw.unit, fw.gauss_raw, noise_n_dev, *fwd_out, *grad_out, graw_main,
@@ -540,12 +539,12 @@ int srf_render_rays_backward(const srf_config* cfg, const srf_pyramid* pyr, cons
   ++g_launches;
   if (int rc = check_cuda("ray_backward")) return rc;
   int l = srf::run_point_mlp_backward_simt(p, *w_main, *grad_main, grad_pyr_chw, fw.pts, fw.viewdir, R * S, S, graw_main, fw.saved_main,
-                                           tf32, mlp_ws, mlp_ws_bytes, st);
+                                           e, mlp_ws, mlp_ws_bytes, st);
   if (l < 0) return fail(SRF_E_WORKSPACE, "srf_render_rays_backward: MLP backward workspace too small");
   g_launches += l;
   if (int rc = check_cuda("main MLP backward")) return rc;
   l = srf::run_point_mlp_backward_simt(p, *w_gauss, *grad_gauss, grad_pyr_chw, fw.gauss_pts, fw.viewdir, R * G, G, graw_gauss,
-                                       fw.saved_gauss, tf32, mlp_ws, mlp_ws_bytes, st);
+                                       fw.saved_gauss, e, mlp_ws, mlp_ws_bytes, st);
   if (l < 0) return fail(SRF_E_WORKSPACE, "srf_render_rays_backward: MLP backward workspace too small");
   g_launches += l;
   return check_cuda("gaussian MLP backward");

@@ -1,9 +1,12 @@
-// float32 SIMT GEMM family used by the strict-precision forward (mlp_simt.cu) and by the backward pass (backward.cu).
+// float32 SIMT GEMM family used by the strict-precision forward and backward of the point MLP (mlp_simt.cu).
 //   C[M x N] = epilogue( sum_k a(m,k) * b(k,n) ),  k ascending, one fmaf chain per output (the summation order does
 //   not depend on the tile shape, so both kernels below give bit-identical results)
 //   AT=false: A stored [M][K] (lda)   AT=true : A stored [K][M] (lda)
 //   BT=true : B stored [N][K] (ldb)   BT=false: B stored [K][N] (ldb)
 //   epilogue: v = acc (+bias[n]); if mask: v = mask[m][n] > 0 ? v : 0; if R: v += R[m][n]; if accumulate: v += C[m][n]
+//   R may alias C (R == C, ldr == ldc): the thread that writes C[m][n] is the only one that reads R[m][n], and it reads
+//   it first, so the residual add works in place (R and C are not __restrict__).  The float32 forward relies on this
+//   (mlp_simt.cu: h = h + lin_z(z) and h = h + fc_1(relu(net)) in one buffer).
 // gemm128_kernel: 128x128x16 tiles, 8x8 outputs per thread, float4 global/shared accesses, register-prefetched double
 // buffering -- the hot one (needs 16-byte aligned rows).  gemm64_kernel: 64x64x16, scalar loads, any shape (lin_in K=42,
 // lin_out M=4 ...).  FP32-FMA-bound: 2*M*N*K flops against SMs (132 on an H100 SXM) x 128 lanes x 2 x clock.

@@ -37,13 +37,6 @@ void launch_upsample_render(const float* depth_xm, const float* color_xm, int gw
 void launch_tsdf_merge(float* tsdf_a, float* weight_a, float* color_a, const float* tsdf_b, const float* weight_b,
                        const float* color_b, long long n, cudaStream_t st);
 
-// mlp_simt.cu : float32 point MLP (gather + positional encoding + ResnetFC), n points in chunks.
-//   pts (n,3) infer-frame points; viewdir (n/n_per,3); raw_out (n,d_out).  Returns number of kernel launches.
-size_t simt_workspace_bytes(int d_latent, int n_points);
-int run_point_mlp_simt(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n,
-                       int n_per, float* raw_out, int32_t* dbg_sphere, void* workspace, size_t ws_bytes,
-                       cudaStream_t st);
-
 // sphere_feature.cu : image-plane feature map -> sphere grid (unet2d_sphere.py:138-166)
 void launch_sphere_feature(const float* x, int C, int h, int w, const float* pix, const long long* pix_sphere, int n, int scale,
                            int oW, int oH, int* winner, float* out, int out_hwc, cudaStream_t st);
@@ -91,7 +84,7 @@ SplitK plan_splitk(const GemmArgs& g, int tiles, int k_gran, int cap);
 void launch_splitk_reduce(const GemmArgs& g, int splits, const SegInfo& sg, cudaStream_t st);
 // SM count of the current device (cached; 132 on an H100 SXM): sizes waves, split-K factors and point chunks
 int device_sm_count();
-// per-thread count of kernels launched by the float32 / tf32 MLP paths (gemm.cu, gemm_tf32.cu, mlp_simt.cu, backward.cu);
+// per-thread count of kernels launched by the float32 / tf32 MLP paths (gemm.cu, gemm_tf32.cu, mlp_simt.cu);
 // the run_* entry points report the difference as their launch count (srf_last_launch_count)
 int& launch_counter();    // 0, or -1 for an operand-layout combination that is not instantiated
 
@@ -99,26 +92,27 @@ int& launch_counter();    // 0, or -1 for an operand-layout combination that is 
 // (at=false, bt=true, no operand ReLU).  Returns 0, or -1 when the shape cannot be expressed as TMA tensor maps.
 int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st);
 
-// one warp per point: X[i] = [ gathered latent (d_latent) | positional encoding (39) | viewdir (3) | 0-pad ], row stride ld
-//   scale_any (5 ints, or NULL): set to 1 for every scale at which some point of the chunk has an in-range bilinear tap.
-//   Scales whose flag stays 0 contribute exact zeros to x_in (quirk Q2: out-of-range normalised coordinates), so the
-//   lin_z GEMMs skip their K-segment -- bit-identical results.
-void launch_build_xin(const DevParams& p, const float* pts, const float* viewdir, int m, int n_per, int point0, float* X, int ld,
-                      int32_t* dbg_sphere, int* scale_any, cudaStream_t st);
-
-// out (M,d_out) = lin_out(relu(Hh))   (resnetfc.py:163; one warp per row)
-void launch_lin_out(const float* Hh, const float* W, const float* bias, float* out, int M, int d_out, cudaStream_t st);
-
-// backward.cu : float32 backward of the path (reference: torch.autograd through scenerf.py:392-748)
-size_t mlp_backward_workspace_bytes(int d_latent, int n_points);
+// mlp_simt.cu : float32 point MLP (gather + positional encoding + ResnetFC) and its backward, n points in chunks.
+//   pts (n,3) infer-frame points; viewdir (n/n_per,3); raw_out (n,d_out).  The run_* functions return the number of
+//   kernel launches, or -1 for a workspace that is too small or an engine the call cannot use.
+// GEMM engine of the chain: SIMT float32 FMAs (gemm.cu), or wgmma tf32 for its NT products (gemm_tf32.cu; training only)
+enum class MatmulEngine { simt, tf32 };
+// workspace of run_point_mlp_simt; save_activations: also enough for a training forward (tf32: its ReLU'd operands)
+size_t simt_workspace_bytes(int d_latent, int n_points, bool save_activations);
 size_t mlp_saved_bytes(int d_latent, int n_points);            // activation store of one pass (SRF_FLAG_SAVE_ACTIVATIONS)
-size_t mlp_forward_save_scratch_bytes(int n_points);           // scratch of run_point_mlp_forward_save (tf32 mode: two ReLU'd operand buffers)
-int run_point_mlp_forward_save(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n, int n_per,
-                               float* raw_out, int32_t* dbg_sphere, void* saved_base, int tf32_matmul, void* scratch, size_t scratch_bytes,
-                               cudaStream_t st);
+size_t mlp_backward_workspace_bytes(int d_latent, int n_points);
+// saved == NULL: inference (SIMT engine only).  saved = a store of mlp_saved_bytes: the training forward, which keeps the
+// activations there for run_point_mlp_backward_simt; raw outputs are bit-identical to inference on the SIMT engine.
+int run_point_mlp_simt(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n, int n_per,
+                       float* raw_out, int32_t* dbg_sphere, void* saved, MatmulEngine e, void* workspace, size_t ws_bytes,
+                       cudaStream_t st);
+// grads: same layout as the weights, pyramid grads CHW; both accumulated into.  saved_base: the store the training
+// forward wrote for the same points, or NULL: the forward is then recomputed chunk by chunk (SIMT engine only).
 int run_point_mlp_backward_simt(const DevParams& p, const srf_mlp_weights& w, const srf_mlp_weights& gw, float* const* grad_pyr_chw,
                                 const float* pts, const float* viewdir, int n, int n_per, const float* g_raw, const void* saved_base,
-                                int tf32_matmul, void* workspace, size_t ws_bytes, cudaStream_t st);
+                                MatmulEngine e, void* workspace, size_t ws_bytes, cudaStream_t st);
+
+// backward.cu : per-ray backward of the compositing (reference: torch.autograd through scenerf.py:392-748)
 void launch_ray_backward(const DevParams& p, int R, const float* raw, const float* t_sorted, const float* unit,
                          const float* gauss_raw, const float* noise_n, const srf_outputs& fwd, const srf_outputs& cot,
                          float* graw_main, float* graw_gauss, cudaStream_t st);

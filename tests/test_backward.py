@@ -266,15 +266,8 @@ def test_cuda_backward_tf32_mode(name):
         name, d, max(w1[0], w2[0], w3[0]), min(w1[1], w2[1], w3[1])))
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("R,matmul", [(1, "fp32"), (150, "fp32"), (150, "tf32")])
-def test_cuda_backward_edge_sizes(R, matmul):
-    """One ray (a single partial tile everywhere) and 150 rays = 9600 sample points = one full 9472-point chunk plus a
-    128-point tail (multi-chunk accumulation, split-K remainders, ragged TMA boxes) against the float64 oracle."""
-    import torch
-    from helpers import hp_from_cfg
-    from oracle import scenerf_oracle as so, backward_oracle as bo
-    from scenerf_b200.autograd import TrainableRenderer, PARAM_KEYS
+def _edge_inputs(R):
+    """R random rays of grad_kitti with seeded noise and a fixed loss (cotangents)."""
     cfg, seed = CASES["grad_kitti"][0](), 43
     pm, pg = synth.make_model_params(cfg)
     pix = synth.random_pixels(50 + R, R, cfg.img_W, cfg.img_H)
@@ -282,16 +275,32 @@ def test_cuda_backward_edge_sizes(R, matmul):
     nu = rng.random((R, cfg.n_pts_uni)).astype(np.float32)
     nn_ = rng.standard_normal((R, cfg.n_gaussians * cfg.n_pts_per_gaussian)).astype(np.float32)
     pyr = synth.make_pyramid(seed, cfg.sphere_W, cfg.sphere_H)
+    cot = {"depth": np.full(R, 0.05, np.float32), "color": np.full((R, 3), 1.0, np.float32), "loss_kl": np.ones(R, np.float32),
+           "gaussian_means": np.full((R, cfg.n_gaussians), 0.01, np.float32)}
+    return cfg, pm, pg, pix, nu, nn_, pyr, cot
+
+
+def edge_case_grads(R, matmul, save_activations=True):
+    """The CUDA gradients of _edge_inputs(R): (main MLP tensors, gaussian MLP tensors, feature maps, renderer)."""
+    import torch
+    from helpers import hp_from_cfg
+    from scenerf_b200.autograd import TrainableRenderer, PARAM_KEYS
+    cfg, pm, pg, pix, nu, nn_, pyr, cot = _edge_inputs(R)
     dev = torch.device("cuda:0")
     mk = lambda d: {k: torch.from_numpy(d[k]).to(dev).requires_grad_(True) for k in PARAM_KEYS}
     tm, tg = mk(pm), mk(pg)
     x_rgb = {k: torch.from_numpy(v).to(dev).requires_grad_(True) for k, v in pyr.items()}
-    t = TrainableRenderer(hp_from_cfg(cfg), tm, tg, device=dev, matmul=matmul)
+    t = TrainableRenderer(hp_from_cfg(cfg), tm, tg, device=dev, save_activations=save_activations, matmul=matmul)
     out = t.render_rays_batch(torch.from_numpy(cfg.K), torch.from_numpy(cfg.T), x_rgb, sampled_pixels=torch.from_numpy(pix),
                               ray_batch_size=R, noise=(torch.from_numpy(nu), torch.from_numpy(nn_)))
-    cot = {"depth": np.full(R, 0.05, np.float32), "color": np.full((R, 3), 1.0, np.float32), "loss_kl": np.ones(R, np.float32),
-           "gaussian_means": np.full((R, cfg.n_gaussians), 0.01, np.float32)}
     sum((out[k] * torch.from_numpy(c).to(dev)).sum() for k, c in cot.items()).backward()
+    return tm, tg, x_rgb, t
+
+
+def check_edge_case(R, matmul, tm, tg, x_rgb):
+    """edge_case_grads against the float64 oracle."""
+    from oracle import scenerf_oracle as so, backward_oracle as bo
+    cfg, pm, pg, pix, nu, nn_, pyr, cot = _edge_inputs(R)
     orc = so.OracleRenderer(cfg, pm, pg)
     r = bo.render_backward(orc, cfg.K, cfg.T, pyr, pix, nu, nn_, cot)
     l2, cos = (0.25, 0.97) if matmul == "tf32" else (2e-2, 0.9995)
@@ -301,3 +310,12 @@ def test_cuda_backward_edge_sizes(R, matmul):
     w2 = _full_tensor_check(tg, r["g_gauss"], "gauss", l2, cos)
     w3 = _full_tensor_check(x_rgb, r["g_pyr"], "maps", l2, cos)
     print("R=%d %s: worst L2-rel %.2e, min cosine %.6f" % (R, matmul, max(w1[0], w2[0], w3[0]), min(w1[1], w2[1], w3[1])))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("R,matmul", [(1, "fp32"), (150, "fp32"), (150, "tf32")])
+def test_cuda_backward_edge_sizes(R, matmul):
+    """One ray (a single partial tile everywhere) and 150 rays = 9600 sample points in one training chunk (split-K
+    remainders, ragged TMA boxes) against the float64 oracle.  test_backward_chunks.py runs the 150-ray case in 10 chunks."""
+    tm, tg, x_rgb, _ = edge_case_grads(R, matmul)
+    check_edge_case(R, matmul, tm, tg, x_rgb)
