@@ -299,12 +299,36 @@ size_t srf_depth_errors_workspace_bytes(void);
 int srf_depth_errors(const float* gt_dev, const float* pred_dev, long long n, void* ws, size_t ws_bytes, double* buckets_dev,
                      int slot, double* frame_dev, void* stream);
 
+/* Novel-view colour metrics (scripts/evaluation/eval_color.py / eval_color_bf.py), DESIGN.md 6.8.  Images are (h,w,3)
+ * row-major float32 in [0,1], as eval_color.py passes them.
+ * srf_psnr_ssim: skimage 0.18.1 peak_signal_noise_ratio(data_range=1) -- 10*log10(1/mse), the squared difference formed in
+ *   float32, inf for identical images -- and structural_similarity(multichannel=True, data_range=1): per channel, 7x7 box
+ *   means in float64, S over the interior [3, h-4] x [3, w-4], mean of the three channel means.  Both sides >= 7 (skimage
+ *   raises below).  frame_dev[2] = (psnr, ssim) if non-NULL; buckets_dev rows of 4 doubles [psnr, ssim, lpips, n]:
+ *   row slot += (psnr, ssim, 0, 1) if non-NULL.  Sums in a fixed order: bit-identical from run to run.  Nothing
+ *   synchronises.  ws: srf_psnr_ssim_workspace_bytes(h, w) bytes (0 for a side below 7).
+ * srf_lpips_vgg: lpips 0.1 LPIPS(net="vgg", version="0.1") of one pair of [0,1] images: the (x-0.5)*2 of compute_lpips,
+ *   the scaling layer (x - shift[c]) / scale[c] (3 host floats each), torchvision VGG16 features[0:30] (13 conv3x3+ReLU on the srf_conv3x3_hwc kernel, 4 max-pools 2x2 floor),
+ *   the head at the five taps (relu1_2 .. relu5_3): f / (sqrt(sum_c f^2) + 1e-10), squared difference, dot lin[k]
+ *   (64/128/256/512/512 floats), spatial mean; *out_dev (one float32) = the sum of the five means.
+ *   w9_dev[13]: [9][Cout][Cin] (tap = ky*3 + kx), values rounded to the nearest tf32 by the caller; Cin = 32 for conv1_1
+ *   (RGB then 29 zero channels), the previous Cout otherwise.  bias_dev[13]: (Cout).  Device pointers 16-byte aligned.
+ *   Sides in [16, 8192].  ws: srf_lpips_workspace_bytes(h, w) bytes.  Nothing synchronises. */
+size_t srf_psnr_ssim_workspace_bytes(int h, int w);
+int srf_psnr_ssim(const float* img_dev, const float* gt_dev, int h, int w, void* ws, size_t ws_bytes, double* buckets_dev, int slot,
+                  double* frame_dev, void* stream);
+size_t srf_lpips_workspace_bytes(int h, int w);
+int srf_lpips_vgg(const float* img0_dev, const float* img1_dev, int h, int w, const float* const* w9_dev, const float* const* bias_dev,
+                  const float* const* lin_dev, const float* shift_host, const float* scale_host, void* ws, size_t ws_bytes, float* out_dev,
+                  void* stream);
+
 /* --- next row: image-side glue of the novel-view sweep (scripts/reconstruction/generate_novel_depths.py:103-152) ---
  * The reference renders an x-major stride-`scale` pixel grid (gw x gh rays, ray = ix*gh + iy), reshapes, transposes
  * and F.interpolate(bilinear)s to (H,W).  srf_upsample_render does that in one pass from the render outputs:
  * depth_xm (gw*gh) -> depth_out (H,W); color_xm (gw*gh,3) -> color_out (H,W,3).  Either pair may be NULL.
  * gw==W && gh==H is the scale-1 case (transpose only).  color_mode: 0 raw, 1 clamp to [0,1] (:144),
- * 2 = the PNG round trip the reference's TSDF stage sees: float32(uint8(c*255))/255*255 (depth2tsdf.py:19-26,98). */
+ * 2 = the PNG round trip the reference's TSDF stage sees: float32(uint8(c*255))/255*255 (depth2tsdf.py:19-26,98),
+ * 3 = the PNG round trip eval_color.py scores: float32(uint8(c*255))/255, in [0,1] (render_colors.py:123-127, eval_color.py:93-94). */
 int srf_upsample_render(const float* depth_xm, const float* color_xm, int gw, int gh, int out_h, int out_w,
                         float* depth_out, float* color_out, int color_mode, void* stream);
 

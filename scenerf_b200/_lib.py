@@ -120,6 +120,13 @@ SYMBOLS = {
                                    C.c_void_p]),
     "srf_upsample_render":(C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_void_p]),
+    "srf_psnr_ssim_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "srf_psnr_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p,
+                                C.c_void_p]),
+    "srf_lpips_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "srf_lpips_vgg": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                C.POINTER(C.c_void_p), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p, C.c_size_t, C.c_void_p,
+                                C.c_void_p]),
     "srf_sphere_feature_dims": (None, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "srf_sphere_feature": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),

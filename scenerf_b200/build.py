@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libscenerf_b200.so")
-SOURCES = ["api.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_tc.cu", "pack.cu", "tsdf.cu", "image_ops.cu", "backward.cu", "gemm.cu", "sphere_feature.cu", "gemm_tf32.cu", "preproj.cu", "conv_tf32.cu", "tma.cu", "mesh.cu", "metrics.cu"]
+SOURCES = ["api.cu", "ray_kernels.cu", "mlp_simt.cu", "mlp_tc.cu", "pack.cu", "tsdf.cu", "image_ops.cu", "backward.cu", "gemm.cu", "sphere_feature.cu", "gemm_tf32.cu", "preproj.cu", "conv_tf32.cu", "tma.cu", "mesh.cu", "metrics.cu", "color_metrics.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*GENCODE, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

@@ -642,7 +642,7 @@ int srf_tsdf_mesh_emit(const float* tsdf_dev, const float* color_dev, const uint
 
 int srf_upsample_render(const float* depth_xm, const float* color_xm, int gw, int gh, int out_h, int out_w,
                         float* depth_out, float* color_out, int color_mode, void* stream) {
-  if (gw < 1 || gh < 1 || out_h < 1 || out_w < 1 || color_mode < 0 || color_mode > 2)
+  if (gw < 1 || gh < 1 || out_h < 1 || out_w < 1 || color_mode < 0 || color_mode > 3)
     return fail(SRF_E_INVALID, "srf_upsample_render: bad shape grid %dx%d -> %dx%d mode %d", gw, gh, out_w, out_h, color_mode);
   if ((!depth_xm || !depth_out) && (!color_xm || !color_out))
     return fail(SRF_E_INVALID, "srf_upsample_render: nothing to do (need a depth pair or a colour pair)");
@@ -711,6 +711,50 @@ int srf_depth_errors(const float* gt_dev, const float* pred_dev, long long n, vo
   srf::launch_depth_errors(gt_dev, pred_dev, n, ws, buckets_dev, slot, frame_dev, (cudaStream_t)stream);
   g_launches = 2;
   return check_cuda("srf_depth_errors");
+}
+
+size_t srf_psnr_ssim_workspace_bytes(int h, int w) { return h >= 7 && w >= 7 ? srf::psnr_ssim_workspace_bytes(h, w) : 0; }
+
+int srf_psnr_ssim(const float* img_dev, const float* gt_dev, int h, int w, void* ws, size_t ws_bytes, double* buckets_dev, int slot,
+                  double* frame_dev, void* stream) {
+  if (!img_dev || !gt_dev) return fail(SRF_E_INVALID, "srf_psnr_ssim: NULL image");
+  // skimage: "win_size exceeds image extent" below a side of 7
+  if (h < 7 || w < 7 || (long long)h * w > 0x7fffffffLL / 3)
+    return fail(SRF_E_INVALID, "srf_psnr_ssim: image %dx%d (each side must be at least 7, the SSIM window)", h, w);
+  if (!buckets_dev && !frame_dev) return fail(SRF_E_INVALID, "srf_psnr_ssim: nothing to write (buckets and frame are NULL)");
+  if (buckets_dev && slot < 0) return fail(SRF_E_INVALID, "srf_psnr_ssim: slot=%d < 0", slot);
+  if (!ws || ws_bytes < srf::psnr_ssim_workspace_bytes(h, w))
+    return fail(SRF_E_WORKSPACE, "srf_psnr_ssim: workspace %zu bytes < %zu", ws_bytes, srf::psnr_ssim_workspace_bytes(h, w));
+  srf::launch_psnr_ssim(img_dev, gt_dev, h, w, ws, buckets_dev, slot, frame_dev, (cudaStream_t)stream);
+  g_launches = 2;
+  return check_cuda("srf_psnr_ssim");
+}
+
+static bool lpips_shape_ok(int h, int w) { return h >= 16 && w >= 16 && h <= 8192 && w <= 8192; }
+
+size_t srf_lpips_workspace_bytes(int h, int w) { return lpips_shape_ok(h, w) ? srf::lpips_workspace_bytes(h, w) : 0; }
+
+int srf_lpips_vgg(const float* img0_dev, const float* img1_dev, int h, int w, const float* const* w9_dev, const float* const* bias_dev,
+                  const float* const* lin_dev, const float* shift_host, const float* scale_host, void* ws, size_t ws_bytes, float* out_dev,
+                  void* stream) {
+  if (!img0_dev || !img1_dev || !w9_dev || !bias_dev || !lin_dev || !shift_host || !scale_host || !out_dev)
+    return fail(SRF_E_INVALID, "srf_lpips_vgg: NULL argument");
+  if (!lpips_shape_ok(h, w))
+    return fail(SRF_E_INVALID, "srf_lpips_vgg: image %dx%d (each side must be in [16, 8192]: four 2x2 pools leave the last tap a pixel)", h, w);
+  for (int i = 0; i < 13; ++i)
+    if (!w9_dev[i] || !bias_dev[i] || !srf::al16(w9_dev[i]) || !srf::al16(bias_dev[i]))
+      return fail(SRF_E_INVALID, "srf_lpips_vgg: conv %d weight / bias NULL or not 16-byte aligned", i);
+  for (int k = 0; k < 5; ++k)
+    if (!lin_dev[k] || !srf::al16(lin_dev[k])) return fail(SRF_E_INVALID, "srf_lpips_vgg: lin%d NULL or not 16-byte aligned", k);
+  if (!srf::al16(ws)) return fail(SRF_E_INVALID, "srf_lpips_vgg: the workspace must be 16-byte aligned");
+  if (!ws || ws_bytes < srf::lpips_workspace_bytes(h, w))
+    return fail(SRF_E_WORKSPACE, "srf_lpips_vgg: workspace %zu bytes < %zu", ws_bytes, srf::lpips_workspace_bytes(h, w));
+  const int l = srf::run_lpips_vgg(img0_dev, img1_dev, h, w, w9_dev, bias_dev, lin_dev, shift_host, scale_host, ws, out_dev,
+                                   (cudaStream_t)stream);
+  if (l == -2) return fail(SRF_E_UNSUPPORTED, "srf_lpips_vgg: cuTensorMapEncodeTiled is not available");
+  if (l < 0) return fail(SRF_E_INVALID, "srf_lpips_vgg: a convolution of the %dx%d image cannot be expressed as tensor maps", h, w);
+  g_launches = l;
+  return check_cuda("srf_lpips_vgg");
 }
 
 int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K, const float* bias,

@@ -32,7 +32,8 @@ __device__ __forceinline__ float blend(float v00, float v01, float v10, float v1
 }
 
 // depth_xm (gw*gh), color_xm (gw*gh,3): ray r = ix*gh + iy (x-major grid).  Outputs row-major (H,W) and (H,W,3).
-// color_mode: 0 raw, 1 clamp to [0,1], 2 PNG round trip ((u8(c*255)/255)*255, a float image in [0,255] as depth2tsdf.py:98 builds)
+// color_mode: 0 raw, 1 clamp to [0,1], 2 PNG round trip ((u8(c*255)/255)*255, a float image in [0,255] as depth2tsdf.py:98 builds),
+// 3 PNG round trip as eval_color.py reads the render back (u8(c*255)/255, in [0,1])
 __global__ void upsample_render_kernel(const float* __restrict__ depth_xm, const float* __restrict__ color_xm, int gw, int gh,
                                        int H, int W, float* __restrict__ depth_out, float* __restrict__ color_out, int color_mode) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -59,9 +60,10 @@ __global__ void upsample_render_kernel(const float* __restrict__ depth_xm, const
     for (int k = 0; k < 3; ++k) {
       float v = c[k];
       if (color_mode >= 1) v = fminf(fmaxf(v, 0.f), 1.f);
-      if (color_mode == 2) {
+      if (color_mode >= 2) {
         const float q = (float)(unsigned char)(int)__fmul_rn(v, 255.f);    // matplotlib to_rgba(bytes=True): (x*255).astype(uint8)
-        v = __fmul_rn(__fdiv_rn(q, 255.f), 255.f);                          // depth2tsdf.py:23,98: float32(u8)/255.0*255.0
+        v = __fdiv_rn(q, 255.f);                                            // eval_color.py:89-94: float32(u8) / 255.0
+        if (color_mode == 2) v = __fmul_rn(v, 255.f);                       // depth2tsdf.py:23,98: float32(u8)/255.0*255.0
       }
       color_out[3 * (size_t)i + k] = v;
     }

@@ -152,6 +152,16 @@ void launch_eval_sc_label(const float* tsdf, long long n, float voxel_size, uint
 size_t depth_errors_workspace_bytes();
 void launch_depth_errors(const float* gt, const float* pred, long long n, void* ws, double* bucket, int slot, double* frame,
                          cudaStream_t st);
+// color_metrics.cu : novel-view colour metrics (eval_color.py): PSNR + SSIM of one (H,W,3) pair (two launches, float64
+// partials in ws, frame = (psnr, ssim), bucket row slot of [psnr, ssim, lpips, n] += (psnr, ssim, -, 1)), and LPIPS-VGG.
+size_t psnr_ssim_workspace_bytes(int H, int W);
+void launch_psnr_ssim(const float* img, const float* gt, int H, int W, void* ws, double* bucket, int slot, double* frame, cudaStream_t st);
+size_t lpips_workspace_bytes(int H, int W);
+// w9[13]: [9][Cout][Cin] tf32-rounded weights (Cin 32 for conv1_1: RGB + zero channels), bias[13], lin[5] (64..512);
+// shift/scale: 3 host floats each.  *out = the pair's LPIPS (float32).  Returns the launch count, or launch_conv3x3_tf32's
+// error (-1 shape, -2 driver entry point missing).
+int run_lpips_vgg(const float* img0, const float* img1, int H, int W, const float* const* w9, const float* const* bias,
+                  const float* const* lin, const float* shift, const float* scale, void* workspace, float* out, cudaStream_t st);
 // image_ops.cu : F.interpolate(size=(out_h,out_w), mode="bilinear", align_corners=False) of one (in_h,in_w) float32 image
 void launch_resize_bilinear(const float* src, int in_h, int in_w, float* dst, int out_h, int out_w, cudaStream_t st);
 

@@ -8,9 +8,10 @@ Reference (file:line):
   scenerf/scripts/reconstruction/generate_sc_gt_bf.py:280-309  the BundleFusion completion target
   scenerf/loss/depth_metrics.py                                compute_depth_errors
   scenerf/scripts/evaluation/save_depth_metrics.py:98-183      ceil(distance) buckets and print_metrics
+  scenerf/scripts/evaluation/eval_color.py:19-110 (+ _bf)      PSNR / SSIM / LPIPS of rendered views, distance buckets
 Counts are integers from one kernel pass, so every statistic equals the reference's to the last bit.  Nothing here
 synchronises the stream except where a host value is returned (get_stats, compute_depth_errors, table, the empty-target
-check of score_reconstruction_kitti)."""
+check of score_reconstruction_kitti, compute_psnr / compute_ssim)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -394,6 +395,160 @@ class DepthErrorBuckets:
             dist.all_gather(sizes, n, group=group)
             self._grow(int(max(int(s.item()) for s in sizes)) - 1)
             self.rows = dist_sum(self.rows, rank, world, group).clone()
+        return self
+
+
+# --- novel-view colour metrics (csrc/color_metrics.cu, DESIGN.md 6.8) ------------------------------------------------
+KITTI_RENDER_SIZE = (407, 124)          # render_colors.py:102-127: the stride-3 grid over 1220x370, (W, H)
+
+
+def gt_color_kitti(img) -> np.ndarray:
+    """eval_color.py:85-87: the source frame (a path or a PIL image) as RGB, resized to 407x124 with PIL's default filter
+    (BICUBIC), as float32 (124,407,3) / 255.  Host I/O on PIL itself, so it is the reference's array exactly."""
+    from PIL import Image
+    im = img if isinstance(img, Image.Image) else Image.open(img)
+    return np.array(im.convert("RGB").resize(KITTI_RENDER_SIZE), dtype=np.float32) / 255.0
+
+
+def gt_color_bf(img) -> np.ndarray:
+    """eval_color_bf.py:85-86: the 640x480 colour frame (a path or a PIL image) as float32 (480,640,3) / 255, not resized."""
+    from PIL import Image
+    im = img if isinstance(img, Image.Image) else Image.open(img)
+    return np.array(im.convert("RGB"), dtype=np.float32) / 255.0
+
+
+def _color_pair(img, gt, device):
+    a, b = torch.as_tensor(img), torch.as_tensor(gt)
+    if a.dim() != 3 or a.shape[2] != 3 or a.shape != b.shape:
+        raise ValueError("expected two (H,W,3) images of one shape, got %s and %s" % (tuple(a.shape), tuple(b.shape)))
+    if a.shape[0] < 7 or a.shape[1] < 7:
+        raise ValueError("win_size exceeds image extent: SSIM needs both sides >= 7, got %dx%d" % (a.shape[0], a.shape[1]))
+    dev = a.device if a.is_cuda else _device(device)
+    return a.to(device=dev, dtype=torch.float32).contiguous(), b.to(device=dev, dtype=torch.float32).contiguous(), dev
+
+
+def _psnr_ssim_call(img, gt, rows, slot, frame, device):
+    lib = _lib.load()
+    a, b, dev = _color_pair(img, gt, device)
+    h, w = int(a.shape[0]), int(a.shape[1])
+    ws_bytes = int(lib.srf_psnr_ssim_workspace_bytes(h, w))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    _lib.check(lib.srf_psnr_ssim(a.data_ptr(), b.data_ptr(), h, w, ws.data_ptr(), ws_bytes, None if rows is None else rows.data_ptr(),
+                                 int(slot), None if frame is None else frame.data_ptr(), _stream(dev)))
+
+
+def _psnr_ssim(img, gt, device):
+    a, b, dev = _color_pair(img, gt, device)
+    frame = torch.empty(2, dtype=torch.float64, device=dev)
+    _psnr_ssim_call(a, b, None, 0, frame, dev)
+    return frame.cpu().numpy()
+
+
+def compute_psnr(img, gt, device=None) -> float:
+    """eval_color.py:19-21: skimage.metrics.peak_signal_noise_ratio(img, gt, data_range=1) of two (H,W,3) float32 images,
+    as a host float (inf for identical images).  Synchronises."""
+    return float(_psnr_ssim(img, gt, device)[0])
+
+
+def compute_ssim(img, gt, device=None) -> float:
+    """eval_color.py:28-30: skimage.metrics.structural_similarity(img, gt, multichannel=True, data_range=1) (0.18.1
+    defaults: 7x7 uniform window, sample covariance), as a host float.  Synchronises."""
+    return float(_psnr_ssim(img, gt, device)[1])
+
+
+def color_bucket_key(dataset: str, source_distance):
+    """The reference's bucket key of one pair.  The distance reaches eval_color*.py through the file name as "{:.2f}": a
+    number is formatted so first, a string is taken as the file name's.  KITTI: math.ceil(float(...)) (3.001 -> "3.00" -> 3,
+    3.006 -> "3.01" -> 4).  BundleFusion: the string itself, never converted to a number."""
+    s = source_distance if isinstance(source_distance, str) else "{:.2f}".format(abs(source_distance))
+    return math.ceil(float(s)) if dataset == "kitti" else s
+
+
+class ColorErrorBuckets:
+    """eval_color.py:96-110 (dataset="kitti") / eval_color_bf.py:90-110 (dataset="bf"): per-pair PSNR, SSIM and LPIPS summed
+    by distance bucket with a pair count, on the device as float64 rows [psnr, ssim, lpips, n].  The bucket key is formed
+    on the host: KITTI math.ceil(float(distance)); BundleFusion the distance string of the file name, "{:.2f}" of the
+    frame difference, never converted to a number (so the table sorts it as a string).  add() never synchronises."""
+
+    def __init__(self, dataset: str = "kitti", device=None):
+        if dataset not in ("kitti", "bf"):
+            raise ValueError("dataset must be 'kitti' or 'bf'")
+        self.dataset = dataset
+        self.device = _device(device)
+        self.keys = {}                               # bucket key -> row
+        self.rows = torch.zeros((0, 4), dtype=torch.float64, device=self.device)
+
+    def _slot(self, key):
+        if key not in self.keys:
+            self.keys[key] = len(self.keys)
+            more = torch.zeros((1, 4), dtype=torch.float64, device=self.device)
+            self.rows = torch.cat([self.rows, more])
+        return self.keys[key]
+
+    def add(self, img, gt, source_distance, lpips=None):
+        """Score one (rendered, ground-truth) pair of (H,W,3) images in [0,1] and add it to its bucket.  lpips: the pair's
+        LPIPS -- a device scalar as LPIPSVGG returns it, or a number -- rounded to float32 (the reference sums
+        lpips_score.item() of a float32 tensor); None leaves the LPIPS column untouched."""
+        slot = self._slot(color_bucket_key(self.dataset, source_distance))
+        _psnr_ssim_call(img, gt, self.rows, slot, None, self.device)
+        if torch.is_tensor(lpips):
+            self.rows[slot, 2] += lpips.to(device=self.device, dtype=torch.float32).to(torch.float64).reshape(())
+        elif lpips is not None:
+            self.rows[slot, 2] += float(np.float32(lpips))
+
+    def merge(self, other: "ColorErrorBuckets"):
+        """Add another set of buckets of the same dataset."""
+        if other.dataset != self.dataset:
+            raise ValueError("cannot merge %s buckets into %s buckets" % (other.dataset, self.dataset))
+        for k, i in other.keys.items():
+            slot = self._slot(k)                     # may grow self.rows
+            self.rows[slot] += other.rows[i].to(self.device)
+        return self
+
+    def as_dicts(self):
+        """(psnr_accum, ssim_accum, lpips_accum, cnt_accum) {key: float / int} in the reference's format."""
+        rows = self.rows.cpu().numpy()
+        out = ({}, {}, {}, {})
+        for k, i in self.keys.items():
+            if rows[i, 3] > 0:
+                for j in range(3):
+                    out[j][k] = float(rows[i, j])
+                out[3][k] = int(rows[i, 3])
+        return out
+
+    def table(self):
+        """print_metrics (eval_color.py:33-60 / eval_color_bf.py:33-60) as text, one line per print."""
+        psnr, ssim, lp, cnt = self.as_dicts()
+        if not cnt:
+            raise ValueError("no pair added")
+        key_fmt = "|{:08d}|" if self.dataset == "kitti" else "|{}|"
+        lines = ["|distance |psnr |ssim   |lpips     |n_frames|"]
+        tp = ts = tl = 0
+        tf = 0
+        for d in sorted(psnr):
+            tp += psnr[d]
+            ts += ssim[d]
+            tl += lp[d]
+            tf += cnt[d]
+            lines.append((key_fmt + "{:02.6f}|{:.6f}|{:.6f}|{:.6f}|").format(d, psnr[d] / cnt[d], ssim[d] / cnt[d], lp[d] / cnt[d], cnt[d]))
+        lines.append("|{}|{:02.6f}|{:.6f}|{:.6f}|{:.6f}|".format("All     ", tp / tf, ts / tf, tl / tf, tf))
+        return "\n".join(lines) + "\n"
+
+    def all_reduce(self, rank: int = 0, world: int = 1, group=None):
+        """Sum the buckets of all ranks in rank order; afterwards every rank holds the same rows bit for bit.  The bucket keys
+        are gathered first (objects), so ranks may have seen different distances."""
+        if world > 1:
+            import torch.distributed as dist
+            keys = [None] * world
+            dist.all_gather_object(keys, list(self.keys), group=group)
+            for ks in keys:
+                for k in ks:
+                    self._slot(k)
+            order = sorted(self.keys)
+            full = torch.stack([self.rows[self.keys[k]] for k in order])
+            summed = dist_sum(full, rank, world, group)
+            self.keys = {k: i for i, k in enumerate(order)}
+            self.rows = summed.clone()
         return self
 
 

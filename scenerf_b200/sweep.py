@@ -53,7 +53,9 @@ def pixel_grid(img_size: Tuple[int, int], scale: int, device) -> Tuple[torch.Ten
     return torch.stack([gx, gy], dim=2).reshape(-1, 2).contiguous(), (int(xs.numel()), int(ys.numel()))
 
 
-COLOR_RAW, COLOR_CLAMP, COLOR_PNG = 0, 1, 2
+# colour of rays_to_images: raw, clamped to [0,1], the PNG round trip of the TSDF stage (x255), the PNG round trip the
+# colour evaluation reads back (float32(uint8(c*255))/255, eval_color.py)
+COLOR_RAW, COLOR_CLAMP, COLOR_PNG, COLOR_EVAL = 0, 1, 2, 3
 
 
 def rays_to_images(depth_rays: Optional[torch.Tensor], color_rays: Optional[torch.Tensor], grid: Tuple[int, int],
@@ -78,22 +80,33 @@ def rays_to_images(depth_rays: Optional[torch.Tensor], color_rays: Optional[torc
     return d_out, c_out
 
 
+# Frames of the colour-render scripts, as NovelDepthSweep arguments: render(T, COLOR_EVAL) gives the image eval_color.py
+# reads back from the saved PNG.
+#   KITTI (render_colors.py:102-127): stride 3 over 1220x370 -> 407x124 rays, transposed, no upsampling.
+#   BundleFusion (render_colors_bf.py:124-163): stride 2 over 640x480, bilinear x2 back to 640x480.
+RENDER_COLORS_KITTI = dict(img_size=(1220, 370), scale=3, ray_batch_size=4000, out_size=(407, 124))
+RENDER_COLORS_BF = dict(img_size=(640, 480), scale=2, ray_batch_size=8000)
+
+
 class NovelDepthSweep:
     """One source frame's sweep: `render(T)` = generate_novel_depths.py:103-152 for one pose (returns device images),
     `reconstruct(...)` = that loop over `rel_poses` feeding depth2tsdf.py:87-103's TSDF volume directly."""
 
     def __init__(self, renderer, cam_K: torch.Tensor, x_rgb: Dict[str, torch.Tensor], img_size=(1220, 370), scale: int = 2,
-                 ray_batch_size: int = 5000):
+                 ray_batch_size: int = 5000, out_size: Optional[Tuple[int, int]] = None):
+        """out_size (W, H) of the images render() returns: img_size (upsampled from the grid) by default; the grid's own
+        size renders without upsampling (render_colors.py)."""
         self.r, self.cam_K, self.x_rgb = renderer, cam_K, x_rgb
         self.img_size, self.scale, self.ray_batch_size = (int(img_size[0]), int(img_size[1])), int(scale), int(ray_batch_size)
         self.pixels, self.grid = pixel_grid(self.img_size, self.scale, renderer.device)
+        self.out_size = self.img_size if out_size is None else (int(out_size[0]), int(out_size[1]))
         self.launches = 0
 
     def render(self, T_source2infer, color_mode: int = COLOR_CLAMP, noise=None):
         out = self.r.render_rays_batch(self.cam_K, T_source2infer, self.x_rgb, ray_batch_size=self.ray_batch_size,
                                        sampled_pixels=self.pixels, noise=noise, outputs="minimal")
         self.launches += self.r.last_launches + 1
-        return rays_to_images(out["depth"], out["color"], self.grid, self.img_size, color_mode)
+        return rays_to_images(out["depth"], out["color"], self.grid, self.out_size, color_mode)
 
     def reconstruct(self, rel_poses: Dict, T_velo2cam, vol_bnds, voxel_size=0.2, trunc_margin=10, noises=None,
                     rank: int = 0, world: int = 1, group=None) -> TSDFVolume:
