@@ -372,11 +372,12 @@ int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, i
                    size_t splitk_ws_floats, int use_tf32, void* stream);
 
 /* Diagnostic (not part of the reference-facing surface): run the tensor-core point MLP of srf_predict but stop each
- * 128-point tile after layer `layer` of the tile program (mlp_tc.cu: 1 lin_in+lin_z0, 2 fc0_0, 4 fc1_0+lin_z1,
+ * 64-point tile after layer `layer` of the tile program (mlp_tc.cu: 1 lin_in+lin_z0, 2 fc0_0, 4 fc1_0+lin_z1,
  * 5 fc0_1, 7 fc1_1+lin_z2, 8 fc0_2, 9 fc1_2, 10 lin_out) and write the raw fp32 accumulator rows to
- * acc_out_dev (ceil(n/128)*128, 512).  With cfg->precision == SRF_PREC_FP32_TC a tile holds 64 points: rows
- * 128t..128t+63 are the high-part products of points 64t..64t+63, rows 128t+64..128t+127 their low-part products,
- * both in units of the weight scale 2^s (acc_out_dev has ceil(n/64)*128 rows). */
+ * acc_out_dev (ceil(n/64)*64, 512): point i at row i.  With cfg->precision == SRF_PREC_FP32_TC acc_out_dev has
+ * ceil(n/32)*64 rows in blocks of 64: point i's complete accumulator (all four hi/lo partial products, in units of
+ * the weight scale 2^s) at row 64 (i/32) + i%32; rows 64 (i/32) + 32..63 (the low-part rows of the former 32-point
+ * tiles) are not written.  Only rows of points i < n are written. */
 int srf_debug_tc_layer(const srf_config* cfg, const srf_pyramid* pyr, const srf_mlp_weights* w,
                        const float* cam_pts_dev, const float* viewdir_dev, int n_cols, int n_per, int layer,
                        float* acc_out_dev, void* workspace_dev, size_t workspace_bytes, void* stream);

@@ -166,7 +166,8 @@ int run_lpips_vgg(const float* img0, const float* img1, int H, int W, const floa
 void launch_resize_bilinear(const float* src, int in_h, int in_w, float* dst, int out_h, int out_w, cudaStream_t st);
 
 // diagnostic: stop every tile after `debug_layer` (1,2,4,5,7,8,9,10 -- see the tile program in mlp_tc.cu) and dump the
-// raw fp32 accumulator (n_tiles*64, 512) to debug_acc
+// raw fp32 accumulator to debug_acc: (n_tiles*64, 512), point i at row i; split mode (ceil(n/32)*64, 512), point i at
+// row 64 (i/32) + i%32 with all four partial products (rows 64 (i/32) + 32..63 untouched); only points i < n
 int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const float* pts, const float* viewdir, int n,
                            int n_per, float* raw_out, int32_t* dbg_sphere, int flags, void* workspace, size_t ws_bytes,
                            int debug_layer, float* debug_acc, cudaStream_t st);

@@ -27,12 +27,14 @@
 // The fp32 hidden state h (64 x 512) does not fit next to the accumulators: it lives in a per-CTA scratch that stays
 // L2-resident, in the accumulator's register order (each thread reads back exactly what it wrote).
 //
-// Split (fp32-grade) mode: every fp32 operand x is carried as fp16 hi = rn(x) and lo = rn(x - hi).  The A tile stacks
-// the two parts of 32 points as ROWS (rows 0-31 hi, rows 32-63 lo -- MMA rows are independent), every weight image is
-// followed by the image of its low parts and both are accumulated into the same registers:
-//   D[r] = x_hi (W_hi + W_lo)^T ,  D[r+32] = x_lo (W_hi + W_lo)^T ,  result[r] = D[r] + D[r+32]   (epilogue)
-// Row r + 32 sits in the thread 64 above the thread of row r, at the same register index: the epilogue hands those
-// partial sums over through the warpgroup's (then idle) latent buffer in shared memory, 32 registers per round.
+// Split (fp32-grade) mode: every fp32 operand x is carried as fp16 hi = rn(x) and lo = rn(x - hi), and the split is
+// carried along K: a tile holds 64 points, every A chunk exists twice (A_hi, A_lo: 64 rows each), every weight image
+// is followed by the image of its low parts, and each image meets both A parts, all into the same registers:
+//   D = A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T + A_lo W_lo^T
+// So each 16 KB image streamed from L2 serves 64 points (the weight stream bounds this kernel), and the epilogue
+// finishes its rows as in fp16 mode.  The ring holds 3 single-image slots per warpgroup; the x chunk and the latent
+// double buffer live in activation chunks that are idle while they are used (Smem<true>, zpass).  Each fc layer sums
+// its K in two halves (flush), which keeps the accumulation round-off at the level of two MMAs per k-step.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -45,9 +47,9 @@
 namespace srf {
 namespace tc {
 
-constexpr int kTileM = 64;                        // MMA rows per tile (points: 64, split mode 32)
+constexpr int kTileM = 64;                        // MMA rows = points per tile (both modes)
 constexpr int kChunkK = 64;                       // fp16 elements per A/B row = 128 bytes = one SW128 atom row
-constexpr int kAChunkBytes = kTileM * 128;        // 8 KB
+constexpr int kAChunkBytes = kTileM * 128;        // 8 KB: one A chunk (split mode: one part of it)
 constexpr int kBRows = 128, kBSlotBytes = kBRows * 128;   // one weight image: 128 rows (N) x 64 k = 16 KB
 constexpr int kHiddenChunks = kHidden / kChunkK;  // 8
 constexpr int kQuarters = kHidden / kBRows;       // 4 N-quarters of 128
@@ -59,22 +61,37 @@ constexpr size_t kHeaderBytes = (size_t)kNumBias * kHidden * sizeof(float);   //
 constexpr int kNumLayers = 11;
 // split-mode blobs: the power-of-two weight scale 2^s and its inverse live in unused entries of the b_out header row
 constexpr int kScaleSlot = 7 * kHidden + 256, kInvScaleSlot = 7 * kHidden + 257;
-// per-CTA scratch (floats): fp32 hidden state (2 warpgroups x 2 quarters x 64 registers x 128 threads), then the
-// split-mode hand-over of the low-part sums of lin_out (the 512-wide layers hand theirs over in shared memory)
+// per-CTA scratch (floats): the fp32 hidden state (2 warpgroups x 2 quarters x 64 registers x 128 threads), then, in
+// split mode, the partial sums of the first half of an fc layer's K loop (same layout; see flush)
 constexpr size_t kScratchFloats = (size_t)2 * kTileM * kHidden;   // 256 KB per CTA
-constexpr size_t kExchangeOffset = (size_t)2 * 2 * 64 * 128;
 
-// dynamic shared memory carve-up
-constexpr int kSmemAct = 0;                                            // 8 A chunks: activations of the current layer
-constexpr int kSmemX = kSmemAct + kHiddenChunks * kAChunkBytes;        // x chunk (positional encoding | view direction)
-constexpr int kSmemZ = kSmemX + kAChunkBytes;                          // 2 latent chunks (double buffer)
-constexpr int kRingBytes = 4 * kBSlotBytes;                            // per warpgroup: 4 fp16 images or 2 hi/lo pairs
-constexpr int kSmemRing = kSmemZ + 2 * kAChunkBytes;
-constexpr int kSmemBar = kSmemRing + 2 * kRingBytes;                   // full[2][4]
-constexpr int kSmemSph = kSmemBar + 2 * 4 * 8;                         // short2 (sx,sy) per point
-constexpr int kSmemMask = kSmemSph + kTileM * 4;                       // active latent chunks of the tile
-constexpr int kSmemTotal = kSmemMask + 16;
-static_assert(kSmemTotal + 1024 <= 232448, "shared memory budget");
+// dynamic shared memory carve-up, per mode.  An A chunk is 64 rows x 64 k; in split mode it is the 8 KB of high parts
+// followed by the 8 KB of low parts, so row r of the low part is row r + 64 of the chunk.
+template <bool SPLIT>
+struct Smem {
+  static constexpr int kParts = SPLIT ? 2 : 1;
+  static constexpr int kAStride = kParts * kAChunkBytes;                      // bytes per A chunk (hi + lo)
+  static constexpr int kAct = 0;                                              // 8 A chunks: activations of the current layer
+  // x chunk (positional encoding | view direction) and the latent double buffer.  fp16: regions of their own.  split:
+  // aliases of activation chunks 0 and 1-2, which no MMA reads while they are in use (see zpass)
+  static constexpr int kX = SPLIT ? kAct : kAct + kHiddenChunks * kAStride;
+  static constexpr int kZ = SPLIT ? kAct + kAStride : kX + kAStride;
+  static constexpr int kSlots = SPLIT ? 3 : 4;                                // per warpgroup, one 16 KB weight image each
+  static constexpr int kRingBytes = kSlots * kBSlotBytes;
+  static constexpr int kRing = SPLIT ? kAct + kHiddenChunks * kAStride : kZ + 2 * kAStride;
+  static constexpr int kBar = kRing + 2 * kRingBytes;                         // full[2][4]
+  static constexpr int kSph = kBar + 2 * 4 * 8;                               // short2 (sx,sy) per point
+  static constexpr int kMask = kSph + kTileM * 4;                             // active latent chunks of the tile
+  static constexpr int kTotal = kMask + 16;
+};
+// the fp16 carve-up: 64 KB activations, 8 KB x, 16 KB latents, 2 x 64 KB rings
+static_assert(Smem<false>::kRing == 88 * 1024 && Smem<false>::kTotal + 1024 <= 232448, "shared memory budget (fp16)");
+// split: 128 KB activations (x and latents inside), 2 x 48 KB rings.  The latent buffers stay clear of the x chunk
+// (lin_in's last MMAs may still read it when lin_z0's first gather starts) and of activation chunk 7 (fc_1's last)
+using SmemSplit = Smem<true>;
+static_assert(SmemSplit::kRing == 128 * 1024 && SmemSplit::kTotal + 1024 <= 232448, "shared memory budget (split)");
+static_assert(SmemSplit::kZ >= SmemSplit::kX + SmemSplit::kAStride &&
+              SmemSplit::kZ + 2 * SmemSplit::kAStride <= SmemSplit::kAct + 7 * SmemSplit::kAStride, "split latent buffers");
 
 struct Layer { int chunks_is_kz, chunks, fresh, signal, is_out; };
 // chunks_is_kz: number of chunks = KZ (runtime) instead of `chunks`
@@ -177,17 +194,19 @@ __device__ __forceinline__ size_t chunk_image_offset(int l, int k, int kz, int p
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Weight stream of one warpgroup.  A stage ("slot") is, for a 512-wide layer, chunk k of one of the warpgroup's two
-// N-quarters (hi + lo images in split mode: contiguous in the blob); for lin_out, the 16 x 64 image(s) of chunk k
-// (warpgroup 0 only).  The order is the tile program's order; lin_z chunks not in the tile's mask are skipped.
+// Weight stream of one warpgroup.  A stage ("slot") is, for a 512-wide layer, one 16 KB image of chunk k: in fp16 mode
+// that of one of the warpgroup's two N-quarters, in split mode the hi or the lo image of one of them (slot j = 2 q +
+// part, the blob's order); for lin_out, the 16 x 64 image(s) of chunk k (hi + lo, 4 KB, in split mode; warpgroup 0
+// only).  The order is the tile program's order; lin_z chunks not in the tile's mask are skipped.
 // ---------------------------------------------------------------------------------------------------------------
+template <int kWideSlots>      // slots per chunk of a 512-wide layer: 2 (fp16) or 4 (split)
 struct Cursor {
   int l = 0, k = 0, j = 0;
   // move to the first slot at or after (l, k, j) that exists; false when the tile's stream is exhausted
   __device__ __forceinline__ bool normalize(int kz, uint64_t mask, int last_layer, int wg) {
     while (l <= last_layer) {
       if (l == kNumLayers - 1 && wg != 0) return false;
-      if (j >= (kLayers[l].is_out ? 1 : 2)) { j = 0; ++k; }
+      if (j >= (kLayers[l].is_out ? 1 : kWideSlots)) { j = 0; ++k; }
       if (k >= layer_chunks(l, kz)) { k = 0; ++l; continue; }
       if (!chunk_active(l, k, mask)) { ++k; continue; }
       return true;
@@ -216,17 +235,20 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
   const uint32_t smem_base = smem_u32(smem);
   const int tid = threadIdx.x;
   const int wg = tid >> 7, t = tid & 127, w = t >> 5, lane = tid & 31;
-  constexpr int kParts = SPLIT ? 2 : 1;                 // weight images per (chunk, quarter): hi (+ lo)
-  constexpr int kPts = SPLIT ? kTileM / 2 : kTileM;     // points per tile
-  constexpr int kSlotBytes = kBSlotBytes * kParts;
-  constexpr int kSlots = kRingBytes / kSlotBytes;       // 4 (fp16) or 2 (split)
-  const uint32_t ring = smem_base + kSmemRing + (uint32_t)wg * kRingBytes;
-  auto full_bar = [&](int s) { return smem_base + kSmemBar + 8u * (uint32_t)(wg * 4 + s); };
-  short2* sph_smem = reinterpret_cast<short2*>(smem + kSmemSph);
-  volatile unsigned long long* mask_smem = reinterpret_cast<volatile unsigned long long*>(smem + kSmemMask);
+  using L = Smem<SPLIT>;
+  constexpr int kParts = L::kParts;                     // weight images per (chunk, quarter) and A parts: hi (+ lo)
+  constexpr int kPts = kTileM;                          // points per tile
+  constexpr int kWideSlots = 2 * kParts;                // ring slots per chunk of a 512-wide layer
+  constexpr int kSlots = L::kSlots;                     // 4 (fp16) or 3 (split)
+  constexpr int kAStride = L::kAStride;
+  constexpr int kSmemAct = L::kAct, kSmemX = L::kX, kSmemZ = L::kZ;
+  const uint32_t ring = smem_base + L::kRing + (uint32_t)wg * L::kRingBytes;
+  auto full_bar = [&](int s) { return smem_base + L::kBar + 8u * (uint32_t)(wg * 4 + s); };
+  short2* sph_smem = reinterpret_cast<short2*>(smem + L::kSph);
+  volatile unsigned long long* mask_smem = reinterpret_cast<volatile unsigned long long*>(smem + L::kMask);
 
   if (tid == 0) {
-    for (int s = 0; s < 8; ++s) mbar_init(smem_base + kSmemBar + 8u * s, 1);
+    for (int s = 0; s < 8; ++s) mbar_init(smem_base + L::kBar + 8u * s, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -237,11 +259,11 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
   const float* bias = reinterpret_cast<const float*>(a.wblob);
   float* scratch = a.scratch + (size_t)blockIdx.x * kScratchFloats;
   float* hbuf = scratch + (size_t)wg * (2 * 64 * 128);             // [j][reg][thread] of this warpgroup
-  float* xbuf = scratch + kExchangeOffset + (size_t)wg * (2 * 64 * 64);   // split: [j][reg][hi thread]
+  [[maybe_unused]] float* pbuf = scratch + (size_t)(2 + wg) * (2 * 64 * 128);       // split: first-half partial sums, same order
   const uint64_t policy = l2_policy_evict_last();
 
   // ---- weight stream: producer (thread 0 of the warpgroup) and consumer positions -----------------------------
-  Cursor pc;
+  Cursor<kWideSlots> pc;
   bool p_live = false;
   uint32_t ppos = 0, cpos = 0, done = 0;                // slots issued / consumed / known complete (whole kernel)
   uint64_t mask = 0;
@@ -249,64 +271,87 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     if (t != 0) return;
     while (p_live && ppos < done + (uint32_t)kSlots) {
       const bool is_out = kLayers[pc.l].is_out != 0;
-      const unsigned char* src = images + chunk_image_offset(pc.l, pc.k, kz, kParts) + (is_out ? 0 : (size_t)(2 * wg + pc.j) * kSlotBytes);
-      const uint32_t bytes = is_out ? (uint32_t)(kOutImgBytes * kParts) : (uint32_t)kSlotBytes;
+      const unsigned char* src = images + chunk_image_offset(pc.l, pc.k, kz, kParts) + (is_out ? 0 : (size_t)(kWideSlots * wg + pc.j) * kBSlotBytes);
+      const uint32_t bytes = is_out ? (uint32_t)(kOutImgBytes * kParts) : (uint32_t)kBSlotBytes;
       const int s = (int)(ppos % kSlots);
       mbar_arrive_expect_tx(full_bar(s), bytes);
-      bulk_g2s(ring + (uint32_t)s * kSlotBytes, src, bytes, full_bar(s), policy);
+      bulk_g2s(ring + (uint32_t)s * kBSlotBytes, src, bytes, full_bar(s), policy);
       ++ppos;
       ++pc.j;
       p_live = pc.normalize(kz, mask, last_layer, wg);
     }
   };
   float acc0[64], acc1[64], acco[8];
-  // wait for the next slot and issue its MMAs: A chunk at a_addr, 4 k-steps of 16 (x hi/lo images)
+  // wait for the next slot and issue its MMAs: A chunk at a_addr, 4 k-steps of 16 (x hi/lo parts in split mode)
   auto wait_slot = [&]() -> uint32_t {
     const int s = (int)(cpos % kSlots);
     mbar_wait<kWatchPointMlp>(full_bar(s), (cpos / kSlots) & 1u, a.error_flag);
-    return ring + (uint32_t)s * kSlotBytes;
+    return ring + (uint32_t)s * kBSlotBytes;
   };
-  // all but the newest commit group have completed: their slots are refilled
+  // all but the newest commit group have completed: their slots are refilled (one commit group per slot)
   auto release1 = [&]() {
     gmma::wait<1>();
     done = cpos - 1;
     produce();
   };
-  auto mma_pair = [&](uint32_t a_addr, bool fresh) {          // both quarters of the warpgroup: 2 slots, 2 commit groups
-    const uint64_t ad = gmma::desc_sw128(a_addr);
-    {
-      const uint32_t b = wait_slot();
-      gmma::fence();
+  // split mode: one weight image (hi or lo part of W) against both parts of the A chunk, into the same registers;
+  // over the image pair of a quarter this is A_hi W_hi + A_lo W_hi + A_hi W_lo + A_lo W_lo.  One slot, one commit group.
+  auto mma_image = [&](float (&acc)[64], uint64_t ad_hi, uint64_t ad_lo, bool fresh) __attribute__((always_inline)) {
+    const uint64_t bd = gmma::desc_sw128(wait_slot());
+    gmma::fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-#pragma unroll
-        for (int part = 0; part < kParts; ++part)
-          gmma::mma_f16_n128(acc0, ad + 2 * k, gmma::desc_sw128(b + part * kBSlotBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
-      gmma::commit();
-      ++cpos;
+    for (int k = 0; k < 4; ++k) {
+      gmma::mma_f16_n128(acc, ad_hi + 2 * k, bd + 2 * k, (fresh && k == 0) ? 0 : 1);
+      gmma::mma_f16_n128(acc, ad_lo + 2 * k, bd + 2 * k, 1);
     }
-    release1();                  // a 2-slot ring (split mode) only holds the second quarter's images once the first slot before it is free
-    {
-      const uint32_t b = wait_slot();
-      gmma::fence();
+    gmma::commit();
+    ++cpos;
+  };
+  auto mma_pair = [&](uint32_t a_addr, bool fresh) {          // both quarters of the warpgroup: 2 slots, 2 commit groups (split: 4, 4)
+    const uint64_t ad = gmma::desc_sw128(a_addr);
+    if constexpr (SPLIT) {
+      const uint64_t ad_lo = gmma::desc_sw128(a_addr + kAChunkBytes);
+      mma_image(acc0, ad, ad_lo, fresh);
+      release1();
+      mma_image(acc0, ad, ad_lo, false);
+      release1();
+      mma_image(acc1, ad, ad_lo, fresh);
+      release1();
+      mma_image(acc1, ad, ad_lo, false);
+    } else {
+      {
+        const uint32_t b = wait_slot();
+        gmma::fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
+        for (int k = 0; k < 4; ++k) gmma::mma_f16_n128(acc0, ad + 2 * k, gmma::desc_sw128(b) + 2 * k, (fresh && k == 0) ? 0 : 1);
+        gmma::commit();
+        ++cpos;
+      }
+      release1();
+      {
+        const uint32_t b = wait_slot();
+        gmma::fence();
 #pragma unroll
-        for (int part = 0; part < kParts; ++part)
-          gmma::mma_f16_n128(acc1, ad + 2 * k, gmma::desc_sw128(b + part * kBSlotBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
-      gmma::commit();
-      ++cpos;
+        for (int k = 0; k < 4; ++k) gmma::mma_f16_n128(acc1, ad + 2 * k, gmma::desc_sw128(b) + 2 * k, (fresh && k == 0) ? 0 : 1);
+        gmma::commit();
+        ++cpos;
+      }
     }
   };
+  // lin_out: one slot (split mode: the hi and lo images, each against both A parts)
   auto mma_out = [&](uint32_t a_addr, bool fresh) {
     const uint64_t ad = gmma::desc_sw128(a_addr);
+    [[maybe_unused]] const uint64_t ad_lo = gmma::desc_sw128(a_addr + kAChunkBytes);
     const uint32_t b = wait_slot();
     gmma::fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k)
 #pragma unroll
-      for (int part = 0; part < kParts; ++part)
-        gmma::mma_f16_n16(acco, ad + 2 * k, gmma::desc_sw128(b + part * kOutImgBytes) + 2 * k, (fresh && k == 0 && part == 0) ? 0 : 1);
+      for (int part = 0; part < kParts; ++part) {
+        const uint64_t bd = gmma::desc_sw128(b + part * kOutImgBytes) + 2 * k;
+        gmma::mma_f16_n16(acco, ad + 2 * k, bd, (fresh && k == 0 && part == 0) ? 0 : 1);
+        if constexpr (SPLIT) gmma::mma_f16_n16(acco, ad_lo + 2 * k, bd, 1);
+      }
     gmma::commit();
     ++cpos;
   };
@@ -319,6 +364,20 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     produce();
   };
   auto sync_all = [&]() { named_bar_sync(1, kThreads); };
+  // split mode: every MMA rounds its sum into the accumulator, and the four products per k-step put twice as many
+  // MMAs on one accumulator as the 32-point row layout did (about sqrt(2) more round-off, measured layer by layer).
+  // Each fc layer therefore sums its K in two halves: after chunk 3 the accumulators go to pbuf and restart from
+  // zero; the epilogue adds the two halves.
+  auto flush = [&]() {
+    retire0();
+#pragma unroll
+    for (int i2 = 0; i2 < 32; ++i2) {
+      reinterpret_cast<float2*>(pbuf)[(size_t)i2 * 128 + t] = make_float2(acc0[2 * i2], acc0[2 * i2 + 1]);
+      reinterpret_cast<float2*>(pbuf)[(size_t)(32 + i2) * 128 + t] = make_float2(acc1[2 * i2], acc1[2 * i2 + 1]);
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+  };
 
   const short2* sph_cur = sph_smem;
   const int erow0 = 16 * w + (lane >> 2);                // accumulator rows of this thread: erow0, erow0 + 8
@@ -356,7 +415,7 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     sync_all();
     mask = PRE ? 0ull : (a.skip_zero ? mask_smem[0] : ~0ull);
     // weight stream of this tile: prime the ring (every slot of the previous tile has completed)
-    pc = Cursor();
+    pc = Cursor<kWideSlots>();
     p_live = pc.normalize(kz, mask, last_layer, wg);
     produce();
 
@@ -527,13 +586,16 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
       cur_scale = -1;
       int c = next_active(kz, mask, -1);
       if (c < 0) return;
+      // split mode: the latent buffers are activation chunks 1-2.  Each warpgroup has retired all but its newest commit
+      // group (chunk 7 of fc_1, or lin_in's x chunk); once both warpgroups are here no MMA reads chunks 1-2 any more
+      if constexpr (SPLIT) sync_all();
       gather(c, smem_base + kSmemZ);
       fence_proxy_async_smem();
       sync_all();
       for (int zi = 0; c >= 0; ++zi) {
         const int cn = next_active(kz, mask, c);
-        mma_pair(smem_base + kSmemZ + (uint32_t)(zi & 1) * kAChunkBytes, false);
-        if (cn >= 0) gather(cn, smem_base + kSmemZ + (uint32_t)((zi + 1) & 1) * kAChunkBytes);
+        mma_pair(smem_base + kSmemZ + (uint32_t)(zi & 1) * kAStride, false);
+        if (cn >= 0) gather(cn, smem_base + kSmemZ + (uint32_t)((zi + 1) & 1) * kAStride);
         retire0();
         fence_proxy_async_smem();
         sync_all();
@@ -546,33 +608,25 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     //   h is kept in register order: element (j, i) of thread t at hbuf[(j * 64 + i) * 128 + t]
     auto epilogue = [&](auto use_h_c, auto write_h_c, auto use_p_c, int bias_idx) __attribute__((always_inline)) {
       constexpr bool USE_H = decltype(use_h_c)::value, WRITE_H = decltype(write_h_c)::value, USE_P = decltype(use_p_c)::value;
+      // split: every epilogue but block 0's E1 (after lin_in + lin_z0) follows an fc layer, whose first half is in pbuf
+      constexpr bool PART = SPLIT && (USE_H || !WRITE_H);
       [[maybe_unused]] const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
-      // split mode: the low-part sums (rows 32-63, threads 64-127 of the warpgroup) go to the thread 64 below through
-      // shared memory, 32 registers per round: the warpgroup's latent buffer (8 KB = 32 registers x 64 threads) is free
-      // in every epilogue -- the MMAs that read it have completed and the next gather comes after the epilogue
-      [[maybe_unused]] float* xs = reinterpret_cast<float*>(smem + kSmemZ + (size_t)wg * kAChunkBytes);   // [reg][hi thread]
+      // split mode: the row is passed through an opaque move so that the swizzled store addresses derived from it are
+      // recomputed in every epilogue; held in registers across the tile (as the compiler would otherwise), they spill
+      int erow = erow0;
+      if constexpr (SPLIT) asm volatile("mov.b32 %0, %0;" : "+r"(erow));
       auto finish = [&](float (&acc)[64], int j) __attribute__((always_inline)) {
 #pragma unroll
-       for (int half = 0; half < 2; ++half) {
-        if constexpr (SPLIT) {
-          if (j | half) named_bar_sync(2 + wg, 128);               // the previous round has been read
-          if (t >= 64) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) xs[i * 64 + (t - 64)] = acc[32 * half + i];
-          }
-          named_bar_sync(2 + wg, 128);
-          if (t >= 64) continue;
-        }
-#pragma unroll
-        for (int i2 = 16 * half; i2 < 16 * half + 16; ++i2) {
+        for (int i2 = 0; i2 < 32; ++i2) {
           const int i = 2 * i2, hh = i2 & 1;
-          const int row = erow0 + 8 * hh;
+          const int row = erow + 8 * hh;
           const int col = 256 * wg + 128 * j + 8 * (i2 >> 1) + ecol;
           float r0 = acc[i], r1 = acc[i + 1];
-          if constexpr (SPLIT) {
-            const float p0 = xs[(i - 32 * half) * 64 + t], p1 = xs[(i + 1 - 32 * half) * 64 + t];
-            r0 = (r0 + p0) * inv_scale; r1 = (r1 + p1) * inv_scale;      // D_hi + D_lo
+          if constexpr (PART) {
+            const float2 f = reinterpret_cast<const float2*>(pbuf)[(size_t)(j * 32 + i2) * 128 + t];
+            r0 += f.x; r1 += f.y;
           }
+          if constexpr (SPLIT) { r0 *= inv_scale; r1 *= inv_scale; }   // the four products are in units of 2^s
           if constexpr (!USE_P) {
             const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + (size_t)bias_idx * kHidden + col));
             r0 += bb.x; r1 += bb.y;
@@ -596,18 +650,17 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
             if constexpr (H16) *hp16 = __floats2half2_rn(r0, r1);
             else *hp = make_float2(r0, r1);
           }
-          const uint32_t addr = smem_base + kSmemAct + (uint32_t)(col >> 6) * kAChunkBytes;
+          const uint32_t addr = smem_base + kSmemAct + (uint32_t)(col >> 6) * kAStride;
           const uint32_t inrow = (uint32_t)((((col & 63) >> 3) ^ (row & 7)) << 4) + (uint32_t)((col & 7) * 2);
           if constexpr (SPLIT) {
             uint32_t hi, lo;
             split_half2(fmaxf(r0, 0.0f), fmaxf(r1, 0.0f), hi, lo);
             sts32(addr + (uint32_t)row * 128 + inrow, hi);
-            sts32(addr + (uint32_t)(row + kPts) * 128 + inrow, lo);
+            sts32(addr + (uint32_t)(row + kPts) * 128 + inrow, lo);     // row r of the low part
           } else {
             sts32(addr + (uint32_t)row * 128 + inrow, pack_relu_half2(r0, r1));
           }
         }
-       }
       };
       finish(acc0, 0);
       finish(acc1, 1);
@@ -621,12 +674,22 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
       fence_proxy_async_smem();
       sync_all();
     };
-    auto dump_acc = [&](bool out) {     // debug: raw accumulator of the current layer
+    // debug: raw accumulator of the current layer.  fp16: row r of tile t to row 64 t + r.  split: the layout of the
+    // former 32-point tiles (hi-part rows, then lo-part rows): point i to row 64 (i / 32) + i % 32, the complete
+    // accumulator (all four products); the low rows stay as the caller left them.  Only points i < n are written.
+    auto dump_acc = [&](bool out, bool part) {
       retire0();
       if (out && wg != 0) return;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        float* dst = a.debug_acc + ((size_t)tile * kTileM + erow0 + 8 * hh) * kHidden;   // split mode: rows 32-63 = low-part products
+        float* dst;
+        if constexpr (SPLIT) {
+          const int gi = row0 + erow0 + 8 * hh;
+          if (gi >= a.n) continue;
+          dst = a.debug_acc + ((size_t)(gi >> 5) * 64 + (gi & 31)) * kHidden;
+        } else {
+          dst = a.debug_acc + ((size_t)tile * kTileM + erow0 + 8 * hh) * kHidden;
+        }
         if (out) {
 #pragma unroll
           for (int c8 = 0; c8 < 2; ++c8) { dst[8 * c8 + ecol] = acco[4 * c8 + 2 * hh]; dst[8 * c8 + ecol + 1] = acco[4 * c8 + 2 * hh + 1]; }
@@ -634,8 +697,17 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
 #pragma unroll
           for (int c8 = 0; c8 < 16; ++c8) {
             const int col = 256 * wg + 8 * c8 + ecol;
-            dst[col] = acc0[4 * c8 + 2 * hh]; dst[col + 1] = acc0[4 * c8 + 2 * hh + 1];
-            dst[col + 128] = acc1[4 * c8 + 2 * hh]; dst[col + 129] = acc1[4 * c8 + 2 * hh + 1];
+            float v[4] = {acc0[4 * c8 + 2 * hh], acc0[4 * c8 + 2 * hh + 1], acc1[4 * c8 + 2 * hh], acc1[4 * c8 + 2 * hh + 1]};
+            if constexpr (SPLIT) {
+              if (part) {                      // the first half of the fc layer's K sum (flush)
+                const int i2 = 2 * c8 + hh;
+                const float2 p0 = reinterpret_cast<const float2*>(pbuf)[(size_t)i2 * 128 + t];
+                const float2 p1 = reinterpret_cast<const float2*>(pbuf)[(size_t)(32 + i2) * 128 + t];
+                v[0] += p0.x; v[1] += p0.y; v[2] += p1.x; v[3] += p1.y;
+              }
+            }
+            dst[col] = v[0]; dst[col + 1] = v[1];
+            dst[col + 128] = v[2]; dst[col + 129] = v[3];
           }
         }
       }
@@ -648,49 +720,48 @@ point_mlp_tc_kernel(const __grid_constant__ DevParams p, const __grid_constant__
     mma_pair(smem_base + kSmemX, true);                           // lin_in
     retire1();
     if (!PRE) zpass();                                            // lin_z0
-    if (a.debug_layer == 1) { dump_acc(false); continue; }
+    if (a.debug_layer == 1) { dump_acc(false, false); continue; }
     bool stop = false;
     for (int b = 0; b < SRF_NUM_BLOCKS; ++b) {
       if (b == 0) epi(F{}, T{}, P{}, b);                          // E1 -> A = relu(h)
       else epi(T{}, T{}, P{}, b);
 #pragma unroll 1
-      for (int k = 0; k < kHiddenChunks; ++k) { mma_pair(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // fc_0
-      if (a.debug_layer == 2 + 3 * b) { dump_acc(false); stop = true; break; }
+      for (int k = 0; k < kHiddenChunks; ++k) {                                                                         // fc_0
+        mma_pair(smem_base + kSmemAct + (uint32_t)k * kAStride, k == 0);
+        retire1();
+        if (SPLIT && k == kHiddenChunks / 2 - 1) flush();
+      }
+      if (a.debug_layer == 2 + 3 * b) { dump_acc(false, true); stop = true; break; }
       epi(F{}, F{}, F{}, 3 + b);                                  // E2 -> A = relu(net)
 #pragma unroll 1
-      for (int k = 0; k < kHiddenChunks; ++k) { mma_pair(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // fc_1
+      for (int k = 0; k < kHiddenChunks; ++k) {                                                                         // fc_1
+        mma_pair(smem_base + kSmemAct + (uint32_t)k * kAStride, k == 0);
+        retire1();
+        if (SPLIT && k == kHiddenChunks / 2 - 1) flush();
+      }
       if (b < SRF_NUM_BLOCKS - 1) {
         if (!PRE) zpass();                                        // lin_z(b+1) accumulates onto fc_1
-        if (a.debug_layer == 4 + 3 * b) { dump_acc(false); stop = true; break; }
-      } else if (a.debug_layer == 9) { dump_acc(false); stop = true; break; }
+        if (a.debug_layer == 4 + 3 * b) { dump_acc(false, true); stop = true; break; }
+      } else if (a.debug_layer == 9) { dump_acc(false, true); stop = true; break; }
     }
     if (stop) continue;
     epi(T{}, F{}, F{}, 6);                                        // E3 -> A = relu(h)
     if (wg == 0) {
 #pragma unroll 1
-      for (int k = 0; k < kHiddenChunks; ++k) { mma_out(smem_base + kSmemAct + (uint32_t)k * kAChunkBytes, k == 0); retire1(); }   // lin_out
-      if (a.debug_layer == 10) { dump_acc(true); continue; }
+      for (int k = 0; k < kHiddenChunks; ++k) { mma_out(smem_base + kSmemAct + (uint32_t)k * kAStride, k == 0); retire1(); }   // lin_out
+      if (a.debug_layer == 10) { dump_acc(true, false); continue; }
       retire0();
       // ---------------- E4: out = ACC[:, :d_out] + b_out ------------------------------------------------------
       const float* bo = bias + (size_t)7 * kHidden;
-      if constexpr (SPLIT) {
-        if (t >= 64) {
+      const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) xbuf[i * 64 + (t - 64)] = acco[i];
-        }
-        named_bar_sync(2, 128);
-      }
-      if (!SPLIT || t < 64) {
-        const float inv_scale = SPLIT ? __ldg(bias + kInvScaleSlot) : 1.0f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int row = erow0 + 8 * ((i >> 1) & 1);
-          const int col = 8 * (i >> 2) + ecol + (i & 1);
-          float v = acco[i];
-          if constexpr (SPLIT) v = (v + xbuf[i * 64 + t]) * inv_scale;
-          const int gi = row0 + row;
-          if (row < kPts && gi < a.n && col < a.d_out) a.raw_out[(size_t)gi * a.d_out + col] = v + __ldg(bo + col);
-        }
+      for (int i = 0; i < 8; ++i) {
+        const int row = erow0 + 8 * ((i >> 1) & 1);
+        const int col = 8 * (i >> 2) + ecol + (i & 1);
+        float v = acco[i];
+        if constexpr (SPLIT) v *= inv_scale;
+        const int gi = row0 + row;
+        if (gi < a.n && col < a.d_out) a.raw_out[(size_t)gi * a.d_out + col] = v + __ldg(bo + col);
       }
     }
   }
@@ -864,7 +935,7 @@ static TcKernelFn tc_kernel(bool h16, bool split, bool pre) { return tc_kernel_a
 constexpr int kMaxTcCtas = 256;
 size_t tc_workspace_bytes(int d_latent, int n_points) {
   (void)d_latent; (void)n_points;
-  // hidden-state / hand-over scratch for up to kMaxTcCtas CTAs + slack
+  // hidden-state / partial-sum scratch for up to kMaxTcCtas CTAs + slack
   return (size_t)kMaxTcCtas * tc::kScratchFloats * sizeof(float) + 256;
 }
 
@@ -874,17 +945,19 @@ int run_point_mlp_tc_debug(const DevParams& p, const srf_mlp_weights& w, const f
   if (ws_bytes < tc_workspace_bytes(p.d_latent, n)) return -1;
   if (debug_layer >= 0 && !(debug_layer < tc::kNumLayers && debug_layer != 0 && debug_layer != 3 && debug_layer != 6))
     return -2;                         // layers without an accumulator-complete point cannot be dumped
-  const size_t smem = tc::kSmemTotal + 1024;
+  const bool split = (flags & kTcFlagSplit) != 0;
+  // + 1 KB: slack for the kernel's round-up to 1024-byte alignment
+  auto smem_of = [](bool s) { return (size_t)(s ? tc::Smem<true>::kTotal : tc::Smem<false>::kTotal) + 1024; };
+  const size_t smem = smem_of(split);
   static bool attr_set = false;
   if (!attr_set) {
-    for (int i = 0; i < kNumTcKernels; ++i) cudaFuncSetAttribute(tc_kernel_at(i), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    for (int i = 0; i < kNumTcKernels; ++i)
+      cudaFuncSetAttribute(tc_kernel_at(i), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of(i % 3 == 2));
     attr_set = true;
   }
-  const bool split = (flags & kTcFlagSplit) != 0;
-  const int tile_pts = split ? tc::kTileM / 2 : tc::kTileM;
   tc::KernelArgs a;
   a.pts = pts; a.viewdir = viewdir; a.n = n; a.n_per = n_per;
-  a.n_tiles = (n + tile_pts - 1) / tile_pts;
+  a.n_tiles = (n + tc::kTileM - 1) / tc::kTileM;
   a.kz = kz_of(p.d_latent);
   a.wblob = reinterpret_cast<const unsigned char*>(split ? w.tc_split_packed : w.tc_packed);
   if (!a.wblob) return -3;

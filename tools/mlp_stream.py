@@ -6,13 +6,13 @@
 Renders config B (453 620 rays x 128 samples, dense, no latent table) with device-side timing of the main pass
 (set_profiling / last_mlp_ms) and prints one JSON line per precision mode:
   * kernel_ms: median main-pass time over --steps renders after --warmup;
-  * tiles: main-pass points / points per tile (32 in fp32tc, 64 in fp16);
+  * tiles: main-pass points / 64 points per tile (both modes);
   * l2_weight_bytes: the bytes of weight images read from L2 per pass.  Every tile streams the whole image region of
     the blob once, so the count is tiles * image bytes (divided by --cluster for a kernel in which a cluster of CTAs
     shares one L2 read of each image);
   * l2_weight_gbs: l2_weight_bytes / kernel time;
-  * tensor_tflops: executed wgmma FLOP (m64n128k16 for the 512-wide layers, m64n16k16 for lin_out, both hi/lo images
-    in fp32tc) / kernel time;
+  * tensor_tflops: executed wgmma FLOP (m64n128k16 for the 512-wide layers, m64n16k16 for lin_out; in fp32tc four
+    products per image pair: both A parts against the hi and the lo image) / kernel time;
   * the GPU's name, power limit and median SM clock, sampled by nvidia-smi during the timed renders.
 --cluster is the number of CTAs that share one L2 read of each image in the library measured (1: the kernel here,
 where every CTA streams its own copy)."""
@@ -80,9 +80,9 @@ def main():
         parts = 2 if split else 1
         images = blob.numel() - HEADER_BYTES - BLOB_SLACK
         wide_chunks = (images // parts - OUT_CHUNKS * OUT_IMG_BYTES) // (4 * IMG_BYTES)   # K-chunks of the 512-wide layers
-        tile_pts = 32 if split else 64
-        tiles = -(-n_points // tile_pts)
-        flop_tile = parts * (wide_chunks * 4 * 4 * (2 * 64 * 128 * 16) + OUT_CHUNKS * 4 * (2 * 64 * 16 * 16))
+        tiles = -(-n_points // 64)
+        products = 4 if split else 1                       # (A_hi, A_lo) x (W_hi, W_lo) in fp32tc
+        flop_tile = products * (wide_chunks * 4 * 4 * (2 * 64 * 128 * 16) + OUT_CHUNKS * 4 * (2 * 64 * 16 * 16))
         r.set_profiling(True)
         for _ in range(args.warmup):
             r.render_rays_batch(K, T, x_rgb, sampled_pixels=pix, outputs="minimal")
