@@ -353,7 +353,8 @@ int srf_sphere_feature(const float* x_chw_dev, int C, int h, int w, const float*
  *   srf_conv3x3_hwc         : y = LeakyReLU_slope( conv3x3(in; dilation = padding = dil) * scale + shift (+ residual) ); slope 1 = none.
  *                             w9_dev: weights repacked [9][Cout][ld_in] (tap = ky*3 + kx; Conv2d.weight[co][ci][ky][kx]), zero for
  *                             padded ci.  Writes out32_dev (H,W,ld32) float32 and/or out16_dev (H,W,ld16) IEEE half -- with
- *                             ld = Cout these ARE the buffers srf_pyramid.hwc[] points to (no CHW->HWC pass).  wgmma tf32
+ *                             ld = Cout these ARE the buffers srf_pyramid.hwc[] points to (no CHW->HWC pass).  One CTA per
+ *                             128-pixel row segment: H * ceil(W/128) must not exceed 65535 (SRF_E_INVALID otherwise).  wgmma tf32
  *                             implicit GEMM, operands read as fp32 with a 10-bit mantissa (cuDNN's default allow_tf32 regime).  The
  *                             tensor core truncates; feed it tensors already rounded to the nearest tf32 value (w9 rounded by the
  *                             caller; round_out != 0 stores out32 rounded because it feeds another convolution; the concat kernel

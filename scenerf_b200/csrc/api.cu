@@ -821,7 +821,7 @@ int srf_conv3x3_hwc(const float* in_dev, int H, int W, int ld_in, const float* w
                                           out32_dev, ld32, out16_dev, ld16, (cudaStream_t)stream);
   if (rc == -2) return fail(SRF_E_UNSUPPORTED, "srf_conv3x3_hwc: cuTensorMapEncodeTiled is not available");
   if (rc) return fail(SRF_E_INVALID, "srf_conv3x3_hwc: shape or alignment not supported (H=%d W=%d ld_in=%d Cout=%d dil=%d; strides must be "
-                                     "multiples of 4 floats, pointers 16-byte aligned)", H, W, ld_in, Cout, dil);
+                                     "multiples of 4 floats, pointers 16-byte aligned, H*ceil(W/128) <= 65535)", H, W, ld_in, Cout, dil);
   g_launches = 1;
   return check_cuda("srf_conv3x3_hwc");
 }

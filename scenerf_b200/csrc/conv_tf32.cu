@@ -121,11 +121,13 @@ __global__ void upsample_concat_kernel(const float* __restrict__ x, int h, int w
 }  // namespace conv
 
 // in: [H][W][Cin] float32 (Cin = channel stride, multiple of 4, 16-byte aligned); w9: [9][Cout][Cin] float32 (tap = ky*3 + kx).
-// Returns 0, -1 (shape / alignment not expressible as tensor maps), -2 (driver entry point missing).
+// Returns 0, -1 (shape / alignment not expressible as tensor maps, or more than 65535 row tiles H * ceil(W/128)), -2 (driver
+// entry point missing).
 int launch_conv3x3_tf32(const float* in, int H, int W, int Cin, const float* w9, int Cout, int dil, const float* scale, const float* shift,
                         const float* residual, int ld_res, float slope, int round_out, float* out32, int ld32, void* out16, int ld16,
                         cudaStream_t st) {
   if (H < 1 || W < 1 || Cin < 4 || (Cin % 4) || Cout < 4 || (Cout % 4) || dil < 1 || !al16(in) || !al16(w9) || !al16(scale) || !al16(shift)) return -1;
+  if ((long long)H * ((W + tf32::kBM - 1) / tf32::kBM) > 65535) return -1;     // one row tile per gridDim.y index (limit 65535)
   if ((out32 && (!al16(out32) || ld32 % 4)) || (out16 && ((reinterpret_cast<uintptr_t>(out16) & 7) || ld16 % 4)) || (residual && (!al16(residual) || ld_res % 4)))
     return -1;
   CUtensorMap tmA, tmB;

@@ -1,7 +1,30 @@
-"""Shared test helpers: build a B200Renderer from a synth.SceneConfig and compare dicts against goldens."""
+"""Shared test helpers: build a B200Renderer from a synth.SceneConfig and compare dicts against goldens; tf32 rounding
+and the accumulation bound of the wgmma .tf32 kernels."""
+import math
+
 import numpy as np
 
 from cases import params_for, pyramid_for
+
+# Accumulation constant of the wgmma .tf32 kernels (conv_tf32.cu, gemm_tf32.cu).  With operands that are tf32 values the
+# products are exact, and an entry's float32 accumulation error stays under
+#   tf32_gamma(K) * sum_k |a_k| |b_k|,   tf32_gamma(K) = TF32_ACC_C * ceil(K / 8) * 2^-24,
+# one rounding per 8-wide k-step of the tensor core.  The accumulator truncates (the unrounded-operand case of
+# tests/test_gpu_conv.py matches a truncating emulation), so a step may lose up to one float32 ulp, 2^-23 of the partial
+# sum: c = 2.  Measured by tests/test_gpu_conv.py on an H100 80GB HBM3 (700 W power limit): c = 1.06 where every operand
+# is >= 0 (Cin = 512, the partial sums grow to S), at most 0.093 on signed operands.
+TF32_ACC_C = 2.0
+
+
+def tf32_gamma(k):
+    return TF32_ACC_C * math.ceil(k / 8) * 2.0 ** -24
+
+
+def tf32_rn(t):
+    """float32 torch tensor -> nearest tf32 value (ties away from zero): the integer trick of decoder.py::_pack and of
+    round_tf32 in conv_tf32.cu."""
+    import torch
+    return ((t.contiguous().view(torch.int32) + 0x1000) & -8192).view(torch.float32)
 
 
 def hp_from_cfg(cfg):

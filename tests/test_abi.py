@@ -81,6 +81,13 @@ def test_argument_validation_of_the_next_rows_without_gpu():
     assert (w.value, h.value) == (94, 28)
     assert lib.srf_sphere_feature(None, 4, 4, 4, None, None, 0, 1, 16, 16, None, 0, None, 0, None) == 1
     assert lib.srf_debug_gemm(None, 4, None, 4, None, 4, 4, 4, 4, None, None, 0, None, 0, 0, None, 0, 1, None) == 1
+    # the convolution launches one CTA per 128-pixel row segment in gridDim.y (at most 65535): a 4096 x 2048 map (65536
+    # segments, inside the sphere grid's 16384 limit) is refused before any tensor map is encoded; the aligned pointers
+    # are never dereferenced
+    p = C.c_void_p(1 << 20)
+    for H, W in ((4096, 2048), (65536, 1), (1, 1 << 30)):
+        rc = lib.srf_conv3x3_hwc(p, H, W, 64, p, 64, 1, p, p, None, 0, 1.0, 0, p, 64, None, 0, None)
+        assert rc == 1 and b"65535" in lib.srf_last_error(), (H, W)
     cfg = _lib.Config()
     cfg.n_gaussians, cfg.n_pts_uni, cfg.n_pts_per_gaussian = 4, 32, 8
     cfg.sphere_W, cfg.sphere_H = 300, 90

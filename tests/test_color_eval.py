@@ -16,7 +16,7 @@ from scenerf_b200 import _lib
 from scenerf_b200.evaluation import color_bucket_key
 
 PSNR_SSIM_SHAPES = ((124, 407), (480, 640), (7, 7), (9, 13))
-LPIPS_SHAPES = ((124, 407), (480, 640), (33, 47))
+LPIPS_SHAPES = ((124, 407), (480, 640), (33, 47), (16, 16))     # 16 x 16: stage 5 convolves a 1 x 1 map (only the centre tap)
 
 
 def u8_image(h, w, seed):
