@@ -116,6 +116,10 @@ typedef struct srf_config {
                                        (float32 storage, 10-bit mantissa operands, float32 accumulate) -- the regime of the
                                        reference's own torch 1.7.1 defaults on Ampere-class GPUs.  Not bit-compatible with
                                        the strict float32 mode; tolerances in DESIGN.md 6.3. */
+#define SRF_FLAG_FP32TC_MATMUL 16   /* float32 path, training (needs SRF_FLAG_SAVE_ACTIVATIONS in the forward): the same GEMMs
+                                       as SRF_FLAG_TF32_MATMUL on tensor cores, as split 3xTF32 products (a_hi b_hi + a_hi b_lo
+                                       + a_lo b_hi, float32 accumulate) of float32-grade accuracy: gradients within the strict
+                                       float32 mode's bounds.  Exclusive with SRF_FLAG_TF32_MATMUL (SRF_E_INVALID); DESIGN.md 6.3. */
 #define SRF_FLAG_SAVE_ACTIVATIONS 4 /* float32 path, training: srf_render_rays keeps the ResnetFC pre-activations of both MLP
                                        passes in its workspace (24.4 KB per sample point) so that srf_render_rays_backward
                                        does not recompute the forward.  Outputs are bit-identical with and without it. */
@@ -366,7 +370,8 @@ int srf_conv3x3_hwc(const float* in_dev, int H, int W, int ld_in, const float* w
                     void* out16_dev, int ld16, void* stream);
 
 /* Diagnostic: one GEMM of the training path, C[M x N] = epilogue(A[M x K] * B[N x K]^T) with float32 device operands.
- * use_tf32 != 0 runs the wgmma tf32 kernel (csrc/gemm_tf32.cu), 0 the float32 SIMT kernel (csrc/gemm.cu).
+ * use_tf32: 0 runs the float32 SIMT kernel (csrc/gemm.cu), 1 the wgmma tf32 kernel (csrc/gemm_tf32.cu), 2 its split
+ * 3xTF32 variant (the SRF_FLAG_FP32TC_MATMUL engine); any other value is SRF_E_INVALID.
  * bias (N) / mask (M x N, keeps values where mask > 0) / residual (M x N) may be NULL; splitk_ws enables split-K. */
 int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K, const float* bias,
                    const float* mask, int ldm, const float* residual, int ldr, int accumulate, float* splitk_ws,
@@ -391,8 +396,8 @@ int srf_last_mlp_ms(float* gauss_ms, float* main_ms);
 
 /* Diagnostic: non-zero once the mbarrier watchdog of a TMA-fed tensor-core kernel fired (readable even after the
  * resulting device trap): 0x40000000 | warp << 24 | (barrier smem offset & 0xFFFFF) << 4 | kernel << 1 | parity, where
- * kernel is 0 for the point MLP (point_mlp_tc_kernel), 1 for the tf32 GEMM (gemm_tf32_nt_kernel) and 2 for the decoder's
- * convolution (conv3x3_tf32_kernel). */
+ * kernel is 0 for the point MLP (point_mlp_tc_kernel), 1 for the tf32 GEMM (gemm_tf32_nt_kernel), 2 for the decoder's
+ * convolution (conv3x3_tf32_kernel) and 3 for the split 3xTF32 GEMM (gemm_tf32_nt_kernel<true>, SRF_FLAG_FP32TC_MATMUL). */
 int srf_debug_watchdog_flag(void);
 
 /* Number of kernels the last srf_render_rays / srf_predict call on this thread launched (bench "gpu_launches"). */

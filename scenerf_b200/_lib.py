@@ -22,6 +22,7 @@ FLAG_SKIP_ZERO_CHUNKS = 1
 FLAG_HIDDEN_FP16 = 2
 FLAG_SAVE_ACTIVATIONS = 4
 FLAG_TF32_MATMUL = 8
+FLAG_FP32TC_MATMUL = 16
 PYR_FP32 = 0
 PYR_FP16 = 1
 

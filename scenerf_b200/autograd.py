@@ -63,6 +63,8 @@ class RenderRaysFunction(torch.autograd.Function):
             cfg.flags |= _lib.FLAG_SAVE_ACTIVATIONS       # the backward reads the pre-activations instead of recomputing them
         if r.tf32_matmul:
             cfg.flags |= _lib.FLAG_SAVE_ACTIVATIONS | _lib.FLAG_TF32_MATMUL
+        elif r.fp32tc_matmul:
+            cfg.flags |= _lib.FLAG_SAVE_ACTIVATIONS | _lib.FLAG_FP32TC_MATMUL
         pyr = r._pack_pyramid(dict(zip(SCALE_KEYS, maps)))
         if pyr.format != _lib.PYR_FP32:
             raise RuntimeError("training needs a renderer built with precision='fp32'")
@@ -142,8 +144,9 @@ class TrainableRenderer:
 
     def __init__(self, hp: dict, mlp, mlp_gaussian, device="cuda:0", rng: str = "torch", save_activations: bool = True,
                  matmul: str = "fp32"):
-        if matmul not in ("fp32", "tf32"):
-            raise ValueError("matmul must be 'fp32' (strict SIMT) or 'tf32' (wgmma tensor cores)")
+        if matmul not in ("fp32", "tf32", "fp32tc"):
+            raise ValueError("matmul must be 'fp32' (strict SIMT), 'tf32' (wgmma tensor cores) or 'fp32tc' (split 3xTF32 wgmma, "
+                             "float32-grade accuracy)")
         state = lambda m: dict(m.named_parameters()) if hasattr(m, "named_parameters") else dict(m)
         self.mlp, self.mlp_gaussian = mlp, mlp_gaussian
         self._state = state
@@ -154,8 +157,10 @@ class TrainableRenderer:
         # False: recompute them chunk by chunk in the backward (less memory, ~25 % more arithmetic)
         self.renderer.save_activations = bool(save_activations)
         # "tf32": the GEMMs of the training forward and of the backward run as wgmma tf32 (float32 storage, 10-bit
-        # mantissa operands) -- several times faster, not bit-compatible with the strict mode (DESIGN.md 6.3)
+        # mantissa operands) -- several times faster, not bit-compatible with the strict mode (DESIGN.md 6.3);
+        # "fp32tc": the same GEMMs on tensor cores as split 3xTF32 products, gradients within the strict mode's bounds
         self.renderer.tf32_matmul = matmul == "tf32"
+        self.renderer.fp32tc_matmul = matmul == "fp32tc"
 
     def render_rays_batch(self, cam_K, T_source2infer, x_rgb, depth_window=100, T_cam2velo=None, sampled_pixels=None,
                           ray_batch_size=128, *, noise=None):

@@ -156,6 +156,17 @@ void prof_record(int which, cudaStream_t st) {
   if (which & 1) g_ev_valid[which >> 1] = true;
 }
 
+// the GEMM engine the matmul flags select (training); validate_matmul has refused both flags together
+srf::MatmulEngine matmul_engine(int flags) {
+  if (flags & SRF_FLAG_FP32TC_MATMUL) return srf::MatmulEngine::fp32tc;
+  return (flags & SRF_FLAG_TF32_MATMUL) ? srf::MatmulEngine::tf32 : srf::MatmulEngine::simt;
+}
+int validate_matmul(const srf_config* cfg, const char* who) {
+  if ((cfg->flags & SRF_FLAG_TF32_MATMUL) && (cfg->flags & SRF_FLAG_FP32TC_MATMUL))
+    return fail(SRF_E_INVALID, "%s: SRF_FLAG_TF32_MATMUL and SRF_FLAG_FP32TC_MATMUL select different GEMM engines; set one", who);
+  return SRF_OK;
+}
+
 int run_mlp(const srf::DevParams& p, int precision, int flags, const srf_mlp_weights& w, const float* pts,
             const float* viewdir, int n, int n_per, float* raw, int32_t* dbg, void* ws, size_t ws_bytes,
             cudaStream_t st, void* saved = nullptr) {
@@ -163,8 +174,8 @@ int run_mlp(const srf::DevParams& p, int precision, int flags, const srf_mlp_wei
   const int pass = (w.d_out == 4) ? 1 : 0;
   prof_record(2 * pass, st);
   if (precision == SRF_PREC_FP32) {
-    // SRF_FLAG_TF32_MATMUL applies to the training forward only
-    const srf::MatmulEngine e = (saved && (flags & SRF_FLAG_TF32_MATMUL)) ? srf::MatmulEngine::tf32 : srf::MatmulEngine::simt;
+    // SRF_FLAG_TF32_MATMUL / SRF_FLAG_FP32TC_MATMUL apply to the training forward only
+    const srf::MatmulEngine e = saved ? matmul_engine(flags) : srf::MatmulEngine::simt;
     l = srf::run_point_mlp_simt(p, w, pts, viewdir, n, n_per, raw, dbg, saved, e, ws, ws_bytes, st);
   } else {
     int f = flags & ~(srf::kTcFlagSplit | srf::kTcFlagPreproj);
@@ -346,6 +357,7 @@ int srf_render_rays(const srf_config* cfg, const srf_pyramid* pyr, const srf_mlp
                     void* stream) {
   g_launches = 0;
   if (int rc = validate(cfg, pyr)) return rc;
+  if (int rc = validate_matmul(cfg, "srf_render_rays")) return rc;
   if (!pyr || !out) return fail(SRF_E_INVALID, "srf_render_rays: pyramid / outputs are NULL");
   if (n_rays == 0) return SRF_OK;                      // empty batch: nothing to write (reference returns empty cats)
   if (n_rays < 0 || !pixels_dev) return fail(SRF_E_INVALID, "srf_render_rays: n_rays=%d pixels=%p", n_rays, (const void*)pixels_dev);
@@ -496,6 +508,7 @@ int srf_render_rays_backward(const srf_config* cfg, const srf_pyramid* pyr, cons
                              size_t workspace_bytes, void* stream) {
   g_launches = 0;
   if (int rc = validate(cfg, pyr)) return rc;
+  if (int rc = validate_matmul(cfg, "srf_render_rays_backward")) return rc;
   if (!pyr || !fwd_out || !grad_out || !grad_main || !grad_gauss || !grad_pyr_chw)
     return fail(SRF_E_INVALID, "srf_render_rays_backward: NULL argument");
   if (cfg->precision != SRF_PREC_FP32 || pyr->format != SRF_PYR_FP32)
@@ -530,10 +543,10 @@ int srf_render_rays_backward(const srf_config* cfg, const srf_pyramid* pyr, cons
   float* graw_gauss = a.take<float>((size_t)R * G * 2);
   const size_t mlp_ws_bytes = workspace_bytes - a.off - 2048;
   void* mlp_ws = a.take<unsigned char>(mlp_ws_bytes);
-  const srf::MatmulEngine e = (cfg->flags & SRF_FLAG_TF32_MATMUL) ? srf::MatmulEngine::tf32 : srf::MatmulEngine::simt;
-  if (e == srf::MatmulEngine::tf32 && !fw.saved_main)
-    return fail(SRF_E_INVALID, "srf_render_rays_backward: SRF_FLAG_TF32_MATMUL needs SRF_FLAG_SAVE_ACTIVATIONS (forward and backward must "
-                               "see the same activations)");
+  const srf::MatmulEngine e = matmul_engine(cfg->flags);
+  if (srf::tensor_cores(e) && !fw.saved_main)
+    return fail(SRF_E_INVALID, "srf_render_rays_backward: %s needs SRF_FLAG_SAVE_ACTIVATIONS (forward and backward must "
+                               "see the same activations)", e == srf::MatmulEngine::tf32 ? "SRF_FLAG_TF32_MATMUL" : "SRF_FLAG_FP32TC_MATMUL");
   srf::launch_ray_backward(p, R, fw.raw, fw.t_sorted, fw.unit, fw.gauss_raw, noise_n_dev, *fwd_out, *grad_out, graw_main,
                            graw_gauss, st);
   ++g_launches;
@@ -761,12 +774,14 @@ int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, i
                    const float* mask, int ldm, const float* residual, int ldr, int accumulate, float* splitk_ws,
                    size_t splitk_ws_floats, int use_tf32, void* stream) {
   if (!A || !B || !C || M < 1 || N < 1 || K < 1) return fail(SRF_E_INVALID, "srf_debug_gemm: bad argument");
+  if (use_tf32 < 0 || use_tf32 > 2) return fail(SRF_E_INVALID, "srf_debug_gemm: use_tf32=%d (0 simt, 1 tf32, 2 split 3xTF32)", use_tf32);
   srf::GemmArgs g;
   g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.bt = true; g.C = C; g.ldc = ldc; g.M = M; g.N = N; g.K = K;
   g.bias = bias; g.mask = mask; g.ldm = ldm; g.R = residual; g.ldr = ldr; g.accumulate = accumulate;
   g.splitk_ws = splitk_ws; g.splitk_ws_floats = splitk_ws_floats;
-  const int rc = use_tf32 ? srf::launch_gemm_tf32(g, (cudaStream_t)stream) : srf::launch_gemm(g, (cudaStream_t)stream);
-  if (rc) return fail(SRF_E_INVALID, "srf_debug_gemm: shape not supported by the %s kernel", use_tf32 ? "tf32" : "simt");
+  const int rc = use_tf32 ? srf::launch_gemm_tf32(g, (cudaStream_t)stream, use_tf32 == 2) : srf::launch_gemm(g, (cudaStream_t)stream);
+  static const char* const kName[3] = {"simt", "tf32", "split 3xTF32"};
+  if (rc) return fail(SRF_E_INVALID, "srf_debug_gemm: shape not supported by the %s kernel", kName[use_tf32]);
   g_launches = 1;
   return check_cuda("srf_debug_gemm");
 }

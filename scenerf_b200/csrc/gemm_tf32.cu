@@ -4,6 +4,8 @@
 // and B through the tf32 tile mainloop of tma.cuh, and the two consumer warpgroups (rows 0-63 / 64-127 of the tile) apply
 // the same epilogue as gemm.cu (bias, ReLU mask, residual, accumulate) straight from registers.  One output tile per CTA;
 // split-K over gridDim.z with fixed-order reduction for the weight-gradient shapes.
+// SPLIT = true is the same kernel on the 3xTF32 mainloop (tma.cuh): hi.hi + hi.lo + lo.hi per k-step, products of
+// float32-grade accuracy from raw float32 operands (the fp32tc training engine); tiles, epilogue and split-K are shared.
 #include "kernels.cuh"
 #include "tma.cuh"
 
@@ -12,6 +14,7 @@ namespace tf32 {
 
 static_assert(kBN == kSegTileN, "segment mode 2 skips whole column tiles of this kernel");
 
+template <bool SPLIT>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* C, int ldc, int M, int N,
                     int K, const float* __restrict__ bias, const float* __restrict__ mask, int ldm, const float* R, int ldr,
@@ -34,7 +37,7 @@ gemm_tf32_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   }
   int k0 = kbeg;                                             // the producer's cursor: first k of the next block
   float acc[64];
-  if (!mainloop<kWatchGemmTf32>(&tmA, &tmB, n_live, err, acc, [&](uint32_t sA, uint32_t sB, uint32_t bar) {
+  if (!mainloop<SPLIT ? kWatchGemmFp32tc : kWatchGemmTf32, SPLIT>(&tmA, &tmB, n_live, err, acc, [&](uint32_t sA, uint32_t sB, uint32_t bar) {
         while (dead(k0)) k0 += kBK;
         tma_load_2d(sA, &tmA, k0, m0, bar);
         tma_load_2d(sB, &tmB, k0, n0, bar);
@@ -76,17 +79,11 @@ static bool encode_f32(CUtensorMap* tm, const float* base, int rows, int K, int 
   return encode_tensor_map_f32(tm, base, 2, dims, strides, box) == 0;
 }
 
-// Only the NT layout with un-transformed operands (at=false, bt=true, no relu_a / relu_b).  Returns 0, or -1 when the
-// shape cannot go through TMA (unaligned rows) -- the caller then falls back to launch_gemm.
-int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st) {
-  if (g.at || !g.bt || g.relu_a || g.relu_b) return -1;
-  if ((g.lda % 4) || (g.ldb % 4) || (g.ldc % 4) || (g.N % 4) || !al16(g.A) || !al16(g.B) || !al16(g.C)) return -1;
-  if ((g.bias && !al16(g.bias)) || (g.mask && (!al16(g.mask) || g.ldm % 4)) || (g.R && (!al16(g.R) || g.ldr % 4))) return -1;
-  if (g.relu_out && (!al16(g.relu_out) || g.ld_relu % 4)) return -1;
-  CUtensorMap tmA, tmB;
-  if (!encode_f32(&tmA, g.A, g.M, g.K, g.lda) || !encode_f32(&tmB, g.B, g.N, g.K, g.ldb)) return -1;
+template <bool SPLIT>
+static int launch(const GemmArgs& g, const CUtensorMap& tmA, const CUtensorMap& tmB, cudaStream_t st) {
+  constexpr size_t smem = SPLIT ? tf32::kSplitSmemBytes : tf32::kSmemBytes;
   static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(tf32::gemm_tf32_nt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tf32::kSmemBytes); attr = true; }
+  if (!attr) { cudaFuncSetAttribute(tf32::gemm_tf32_nt_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
   int* err = watchdog_device_flag();
   dim3 grid((g.N + tf32::kBN - 1) / tf32::kBN, (g.M + tf32::kBM - 1) / tf32::kBM);
   SegInfo sg;
@@ -96,17 +93,29 @@ int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st) {
   const SplitK sk = g.relu_out ? SplitK{1, g.K} : plan_splitk(g, grid.x * grid.y, tf32::kBK, 32);
   if (sk.splits > 1) {
     grid.z = sk.splits;
-    tf32::gemm_tf32_nt_kernel<<<grid, tf32::kThreads, tf32::kSmemBytes, st>>>(tmA, tmB, g.splitk_ws, g.N, g.M, g.N, g.K, nullptr, nullptr, 0,
-                                                                             nullptr, 0, 0, sk.k_per, g.skip_if_zero, sg, err, nullptr, 0);
+    tf32::gemm_tf32_nt_kernel<SPLIT><<<grid, tf32::kThreads, smem, st>>>(tmA, tmB, g.splitk_ws, g.N, g.M, g.N, g.K, nullptr, nullptr, 0,
+                                                                        nullptr, 0, 0, sk.k_per, g.skip_if_zero, sg, err, nullptr, 0);
     launch_splitk_reduce(g, sk.splits, sg, st);
     launch_counter() += 2;
   } else {
     ++launch_counter();
-    tf32::gemm_tf32_nt_kernel<<<grid, tf32::kThreads, tf32::kSmemBytes, st>>>(tmA, tmB, g.C, g.ldc, g.M, g.N, g.K, g.bias, g.mask, g.ldm, g.R,
-                                                                             g.ldr, g.accumulate, g.K, g.skip_if_zero, sg, err, g.relu_out,
-                                                                             g.ld_relu);
+    tf32::gemm_tf32_nt_kernel<SPLIT><<<grid, tf32::kThreads, smem, st>>>(tmA, tmB, g.C, g.ldc, g.M, g.N, g.K, g.bias, g.mask, g.ldm, g.R,
+                                                                        g.ldr, g.accumulate, g.K, g.skip_if_zero, sg, err, g.relu_out,
+                                                                        g.ld_relu);
   }
   return 0;
+}
+
+// Only the NT layout with un-transformed operands (at=false, bt=true, no relu_a / relu_b).  Returns 0, or -1 when the
+// shape cannot go through TMA (unaligned rows) -- the caller then falls back to launch_gemm.
+int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st, bool split) {
+  if (g.at || !g.bt || g.relu_a || g.relu_b) return -1;
+  if ((g.lda % 4) || (g.ldb % 4) || (g.ldc % 4) || (g.N % 4) || !al16(g.A) || !al16(g.B) || !al16(g.C)) return -1;
+  if ((g.bias && !al16(g.bias)) || (g.mask && (!al16(g.mask) || g.ldm % 4)) || (g.R && (!al16(g.R) || g.ldr % 4))) return -1;
+  if (g.relu_out && (!al16(g.relu_out) || g.ld_relu % 4)) return -1;
+  CUtensorMap tmA, tmB;
+  if (!encode_f32(&tmA, g.A, g.M, g.K, g.lda) || !encode_f32(&tmB, g.B, g.N, g.K, g.ldb)) return -1;
+  return split ? launch<true>(g, tmA, tmB, st) : launch<false>(g, tmA, tmB, st);
 }
 
 }  // namespace srf

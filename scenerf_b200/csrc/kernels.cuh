@@ -45,7 +45,8 @@ inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) =
 
 // Mapped host flag of the mbarrier watchdog of the sm_90a kernels (tma.cuh), readable even after the resulting device
 // trap: 0, or 0x40000000 | warp << 24 | (barrier smem offset & 0xFFFFF) << 4 | kernel << 1 | parity, where kernel is
-// 0 for point_mlp_tc_kernel, 1 for gemm_tf32_nt_kernel and 2 for conv3x3_tf32_kernel.
+// 0 for point_mlp_tc_kernel, 1 for gemm_tf32_nt_kernel, 2 for conv3x3_tf32_kernel and 3 for the split (3xTF32)
+// gemm_tf32_nt_kernel.
 int watchdog_flag();
 int* watchdog_device_flag();   // the device address the kernels write (allocated on first use; null if that failed)
 
@@ -89,14 +90,18 @@ int device_sm_count();
 int& launch_counter();    // 0, or -1 for an operand-layout combination that is not instantiated
 
 // gemm_tf32.cu : the same contract on tensor cores (wgmma .tf32, float32 operands read in place); NT layout only
-// (at=false, bt=true, no operand ReLU).  Returns 0, or -1 when the shape cannot be expressed as TMA tensor maps.
-int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st);
+// (at=false, bt=true, no operand ReLU).  split: the 3xTF32 kernel (hi.hi + hi.lo + lo.hi, float32-grade products).
+// Returns 0, or -1 when the shape cannot be expressed as TMA tensor maps.
+int launch_gemm_tf32(const GemmArgs& g, cudaStream_t st, bool split = false);
 
 // mlp_simt.cu : float32 point MLP (gather + positional encoding + ResnetFC) and its backward, n points in chunks.
 //   pts (n,3) infer-frame points; viewdir (n/n_per,3); raw_out (n,d_out).  The run_* functions return the number of
 //   kernel launches, or -1 for a workspace that is too small or an engine the call cannot use.
-// GEMM engine of the chain: SIMT float32 FMAs (gemm.cu), or wgmma tf32 for its NT products (gemm_tf32.cu; training only)
-enum class MatmulEngine { simt, tf32 };
+// GEMM engine of the chain: SIMT float32 FMAs (gemm.cu), or for its NT products wgmma tf32 (gemm_tf32.cu) or the split
+// 3xTF32 wgmma kernel of float32-grade accuracy (fp32tc); the two tensor-core engines are training only and arrange the
+// operands the same way.
+enum class MatmulEngine { simt, tf32, fp32tc };
+inline bool tensor_cores(MatmulEngine e) { return e != MatmulEngine::simt; }
 // workspace of run_point_mlp_simt; save_activations: also enough for a training forward (tf32: its ReLU'd operands)
 size_t simt_workspace_bytes(int d_latent, int n_points, bool save_activations);
 size_t mlp_saved_bytes(int d_latent, int n_points);            // activation store of one pass (SRF_FLAG_SAVE_ACTIVATIONS)

@@ -3,7 +3,8 @@
 // This is the STRICT mode (srf_precision::SRF_PREC_FP32): every multiply-add is an fp32 FMA, so it tracks the
 // reference (cuBLAS/MKL sgemm, scenerf/models/resnetfc.py:133-164) to float32 round-off.  It is also the device-side
 // yardstick the tensor-core kernel is compared against at sizes the CPU oracle cannot reach, and the forward and backward
-// of training (SRF_FLAG_TF32_MATMUL moves the NT products of training onto the wgmma tf32 kernel, gemm_tf32.cu).
+// of training (SRF_FLAG_TF32_MATMUL moves the NT products of training onto the wgmma tf32 kernel, gemm_tf32.cu;
+// SRF_FLAG_FP32TC_MATMUL onto its split 3xTF32 variant, which keeps float32-grade products).
 //
 // Every decision about how the ResnetFC chain is sequenced lives here: the chunk sizes of inference and training, the
 // layout of the saved activations, ONE forward (inference, training forward and the backward's recompute) and ONE
@@ -228,7 +229,8 @@ static void transpose(const float* src, int lds, int rows, int cols, float* dst,
 }
 
 // One GEMM of the chain: C[M x N] = epilogue(op(A) op(B)) with gemm.cu's operand layouts; g carries the epilogue and
-// scratch fields.  MatmulEngine::tf32 puts an NT product without operand ReLU on the wgmma kernel; every other product,
+// scratch fields.  A tensor-core engine puts an NT product without operand ReLU on the wgmma kernel (fp32tc: its split
+// 3xTF32 variant); every other product,
 // and a shape that kernel cannot take, runs on the SIMT kernels, and relu_out is then filled by a separate pass over C
 // (the callers keep ldc == ld_relu == N).
 template <bool AT, bool BT, bool RA = false, bool RB = false>
@@ -236,7 +238,7 @@ static void gemm(const float* A, int lda, const float* B, int ldb, float* C, int
                  cudaStream_t st) {
   g.A = A; g.lda = lda; g.at = AT; g.relu_a = RA; g.B = B; g.ldb = ldb; g.bt = BT; g.relu_b = RB;
   g.C = C; g.ldc = ldc; g.M = M; g.N = N; g.K = K;
-  if (e == MatmulEngine::tf32 && launch_gemm_tf32(g, st) == 0) return;
+  if (tensor_cores(e) && launch_gemm_tf32(g, st, e == MatmulEngine::fp32tc) == 0) return;
   launch_gemm(g, st);
   if (g.relu_out) {
     const size_t n4 = (size_t)M * N / 4;
@@ -286,7 +288,7 @@ static Acts saved_view(void* base, int d_latent, int n) {
   return a;
 }
 
-// the training forward keeps its activations in the store; on the tf32 engine it needs two ReLU'd operand buffers per chunk
+// the training forward keeps its activations in the store; on a tensor-core engine it needs two ReLU'd operand buffers per chunk
 static size_t relu_scratch_bytes(int n_points) {
   return (size_t)2 * (size_t)(n_points < train_chunk() ? n_points : train_chunk()) * kHidden * sizeof(float) + 256;
 }
@@ -302,12 +304,12 @@ size_t simt_workspace_bytes(int d_latent, int n_points, bool save_activations) {
 // block PRE[b] = h + lin_z[b](z), NET[b] = fc_0(relu(PRE[b])), h = PRE[b] + fc_1(relu(NET[b])); H3 = h after block 2.
 // The residual always enters as the epilogue's R operand, which gemm.cu allows to alias C, so inference runs the same
 // arithmetic in two buffers (PRE[b] = H3 = h, NET[b] = net) and training keeps every activation apart.
-// tf32: relu_scratch holds 2 x m x 512 floats -- the tensor-core GEMM reads its A operand as stored, so the producing
+// tf32 / fp32tc: relu_scratch holds 2 x m x 512 floats -- the tensor-core GEMM reads its A operand as stored, so the producing
 // GEMM's epilogue also stores the ReLU'd activations the next GEMM consumes.
 static void resnetfc_forward(const DevParams& p, const srf_mlp_weights& w, const Acts& a, int ld, int m, MatmulEngine e,
                              float* relu_scratch, cudaStream_t st) {
   const int H = kHidden, DL = p.d_latent;
-  const bool tc = e == MatmulEngine::tf32;
+  const bool tc = tensor_cores(e);
   GemmArgs o;
   o.bias = w.lin_in_b;
   gemm<false, true>(a.X + DL, ld, w.lin_in_w, kDX, a.PRE[0], H, m, H, kDX, o, e, st);                        // h = lin_in(x)
@@ -345,7 +347,7 @@ int run_point_mlp_simt(const DevParams& p, const srf_mlp_weights& w, const float
   Acts a;
   float* relu_scratch = nullptr;
   if (saved) {                             // training forward: the activations of the whole pass go to the store
-    if (e == MatmulEngine::tf32) {
+    if (tensor_cores(e)) {
       if (ws_bytes < relu_scratch_bytes(n)) return -1;
       relu_scratch = reinterpret_cast<float*>(workspace);
     }
@@ -374,22 +376,22 @@ int run_point_mlp_simt(const DevParams& p, const srf_mlp_weights& w, const float
 // ---------------------------------------------------------------------------------------------------------------
 size_t mlp_backward_workspace_bytes(int d_latent, int n_points) {
   const size_t m = (size_t)(n_points < train_chunk() ? n_points : train_chunk());
-  // + tf32 mode: transposed copies (2 x [512][m], X^T [ld][m]) and the transposed weights (6 x 512x512, 3 x 512 x d_latent)
+  // + tensor-core engines: transposed copies (2 x [512][m], X^T [ld][m]) and the transposed weights (6 x 512x512, 3 x 512 x d_latent)
   const size_t tf32_extra = ((size_t)2 * kHidden * (m + 4) + (size_t)xin_ld(d_latent) * (m + 4) + (size_t)6 * kHidden * kHidden +
                              (size_t)3 * kHidden * d_latent) * sizeof(float);
   return m * ((size_t)2 * xin_ld(d_latent) + 10 * kHidden) * sizeof(float) + kSplitKFloats * sizeof(float) + 512 + tf32_extra;
 }
 
 // The products of the backward chain, each written once for both engines.  SIMT: TN / NN kernels on the activations and
-// weights as stored.  tf32: every product is NT -- dW = (dY^T)(relu(X)^T)^T with K = m from transposed copies of the
+// weights as stored.  tf32 / fp32tc: every product is NT -- dW = (dY^T)(relu(X)^T)^T with K = m from transposed copies of the
 // chunk, dX = dY (W^T)^T from the transposed weights.
 struct ChainBackward {
   const DevParams& p;
   MatmulEngine e;
   int m, mq;                 // rows of the chunk; row stride of the transposed copies (16-byte aligned rows)
   float* SK;                 // split-K scratch
-  float* Tt0; float* Tt1;    // tf32: dY^T, relu(X)^T
-  const float* Xt;           // tf32: z^T of the chunk
+  float* Tt0; float* Tt1;    // tensor cores: dY^T, relu(X)^T
+  const float* Xt;           // tensor cores: z^T of the chunk
   cudaStream_t st;
 
   GemmArgs accumulate_splitk() const {
@@ -400,7 +402,7 @@ struct ChainBackward {
   // gW[M x N] += dY[m x M]^T relu?(X)[m x N]
   template <bool RELU>
   void wgrad(const float* dY, int ldy, const float* X, int ldx, float* gW, int M, int N, MatmulEngine eng) const {
-    if (eng == MatmulEngine::tf32) {
+    if (tensor_cores(eng)) {
       transpose<false>(dY, ldy, m, M, Tt0, mq, st);
       transpose<RELU>(X, ldx, m, N, Tt1, mq, st);
       gemm<false, true>(Tt0, mq, Tt1, mq, gW, N, M, N, m, accumulate_splitk(), eng, st);
@@ -414,16 +416,16 @@ struct ChainBackward {
     GemmArgs o;
     o.mask = mask; o.ldm = H;
     if (R) { o.R = R; o.ldr = H; }
-    if (e == MatmulEngine::tf32) gemm<false, true>(dY, H, WT, H, dX, H, m, H, H, o, e, st);
+    if (tensor_cores(e)) gemm<false, true>(dY, H, WT, H, dX, H, m, H, H, o, e, st);
     else gemm<false, false>(dY, H, W, H, dX, H, m, H, H, o, e, st);
   }
   // lin_z, whose input is the latent z (the first d_latent columns of X): gW += dY^T z, then dZ (+)= dY W (W = lin_z
-  // weight, WT = W^T).  SIMT: both products per pyramid scale, a scale no point reaches returning at its flag; tf32: one
+  // weight, WT = W^T).  SIMT: both products per pyramid scale, a scale no point reaches returning at its flag; tensor cores: one
   // launch each, the kernel skipping the column tiles of such scales.
   void latent(const float* dY, const float* X, int ld, const float* W, const float* WT, float* gW, float* dZ, int accumulate,
               const int* flags) const {
     const int H = kHidden, DL = p.d_latent;
-    if (e == MatmulEngine::tf32) {
+    if (tensor_cores(e)) {
       transpose<false>(dY, H, m, H, Tt0, mq, st);
       GemmArgs o = accumulate_splitk();
       set_segments(o, flags, 2, p.ch_off);
@@ -447,7 +449,7 @@ int run_point_mlp_backward_simt(const DevParams& p, const srf_mlp_weights& w, co
                                 const float* pts, const float* viewdir, int n, int n_per, const float* g_raw, const void* saved_base,
                                 MatmulEngine e, void* workspace, size_t ws_bytes, cudaStream_t st) {
   if (ws_bytes < mlp_backward_workspace_bytes(p.d_latent, n)) return -1;
-  if (!saved_base && e != MatmulEngine::simt) return -1;   // the recompute is the SIMT chain: tf32 gradients need the tf32 forward's store
+  if (!saved_base && tensor_cores(e)) return -1;   // the recompute is the SIMT chain: tensor-core gradients need that engine's forward store
   const int ld = xin_ld(p.d_latent), H = kHidden, DL = p.d_latent;
   const size_t cap = (size_t)(n < train_chunk() ? n : train_chunk());
   Acts chunk_acts;                                         // recompute buffers of one chunk
@@ -462,14 +464,14 @@ int run_point_mlp_backward_simt(const DevParams& p, const srf_mlp_weights& w, co
   float* SK = q; q += kSplitKFloats;
   chunk_acts.flags = reinterpret_cast<int*>(q); q += 128;
   chunk_acts.whole_pass = false;
-  // tf32 mode scratch
+  // tensor-core engines' scratch
   const int mp = (int)((cap + 3) / 4 * 4);
   float* Tt0 = q; q += (size_t)H * mp;
   float* Tt1 = q; q += (size_t)H * mp;
   float* Xt = q; q += (size_t)ld * mp;
   float* WT0[3]; float* WT1[3]; float* WTZ[3];
   for (int b = 0; b < 3; ++b) { WT0[b] = q; q += (size_t)H * H; WT1[b] = q; q += (size_t)H * H; WTZ[b] = q; q += (size_t)H * DL; }
-  if (e == MatmulEngine::tf32) {
+  if (tensor_cores(e)) {
     for (int b = 0; b < 3; ++b) {                          // W^T so that dX = dY W becomes an NT product
       transpose<false>(w.fc0_w[b], H, H, H, WT0[b], H, st);
       transpose<false>(w.fc1_w[b], H, H, H, WT1[b], H, st);
@@ -495,7 +497,7 @@ int run_point_mlp_backward_simt(const DevParams& p, const srf_mlp_weights& w, co
     colsum(g_out, w.d_out, m, w.d_out, G(gw.lin_out_b), SK, st);
     lin_out_dx_kernel<<<(m * H + 255) / 256, 256, 0, st>>>(g_out, w.d_out, w.lin_out_w, a.H3, dH, m);
     ++launch_counter();
-    if (e == MatmulEngine::tf32) transpose<false>(a.X, ld, m, DL, Xt, bw.mq, st);                            // z^T, once per chunk
+    if (tensor_cores(e)) transpose<false>(a.X, ld, m, DL, Xt, bw.mq, st);                            // z^T, once per chunk
     for (int b = 2; b >= 0; --b) {
       bw.wgrad<true>(dH, H, a.NET[b], H, G(gw.fc1_w[b]), H, H, e);                                           // gW_fc1 += dh^T relu(net)
       colsum(dH, H, m, H, G(gw.fc1_b[b]), SK, st);

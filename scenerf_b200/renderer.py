@@ -119,6 +119,7 @@ class B200Renderer:
         self.last_backward_launches = 0
         self.save_activations = False
         self.tf32_matmul = False
+        self.fp32tc_matmul = False
 
     # ------------------------------------------------------------------------------------------------------------
     @classmethod
