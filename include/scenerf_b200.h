@@ -380,10 +380,14 @@ int srf_debug_gemm(const float* A, int lda, const float* B, int ldb, float* C, i
 /* Diagnostic (not part of the reference-facing surface): run the tensor-core point MLP of srf_predict but stop each
  * 64-point tile after layer `layer` of the tile program (mlp_tc.cu: 1 lin_in+lin_z0, 2 fc0_0, 4 fc1_0+lin_z1,
  * 5 fc0_1, 7 fc1_1+lin_z2, 8 fc0_2, 9 fc1_2, 10 lin_out) and write the raw fp32 accumulator rows to
- * acc_out_dev (ceil(n/64)*64, 512): point i at row i.  With cfg->precision == SRF_PREC_FP32_TC acc_out_dev has
- * ceil(n/32)*64 rows in blocks of 64: point i's complete accumulator (all four hi/lo partial products, in units of
- * the weight scale 2^s) at row 64 (i/32) + i%32; rows 64 (i/32) + 32..63 (the low-part rows of the former 32-point
- * tiles) are not written.  Only rows of points i < n are written. */
+ * acc_out_dev (ceil(n/64)*64, 512): point i at row i; the rows n..ceil(n/64)*64-1 of the last tile hold the
+ * accumulators of its zero-padded rows (no point, no latent taps).  With cfg->precision == SRF_PREC_FP32_TC
+ * acc_out_dev has ceil(n/32)*64 rows in blocks of 64: point i's complete accumulator (all four hi/lo partial
+ * products, in units of the weight scale 2^s) at row 64 (i/32) + i%32; rows 64 (i/32) + 32..63 (the low-part rows
+ * of the former 32-point tiles) and the rows of points i >= n are not written.  Layer 10 writes columns 0..15 only.
+ * The pass is the one srf_predict runs for w: when pyr carries the latent table of w's network (latent_table for
+ * d_out 4, latent_table_gauss otherwise) the table variant of the kernel runs, whose layers 1, 4 and 7 then hold
+ * lin_in only / fc_1 only. */
 int srf_debug_tc_layer(const srf_config* cfg, const srf_pyramid* pyr, const srf_mlp_weights* w,
                        const float* cam_pts_dev, const float* viewdir_dev, int n_cols, int n_per, int layer,
                        float* acc_out_dev, void* workspace_dev, size_t workspace_bytes, void* stream);

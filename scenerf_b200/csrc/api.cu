@@ -167,6 +167,17 @@ int validate_matmul(const srf_config* cfg, const char* who) {
   return SRF_OK;
 }
 
+// the tensor-core pass of network w: its flags (split mode, latent table) and its DevParams.  A latent table belongs to
+// one network: the main pass (d_out 4) reads latent_table, the proposal pass latent_table_gauss
+int tc_pass(const srf::DevParams& p, int precision, int flags, const srf_mlp_weights& w, srf::DevParams& pp) {
+  int f = flags & ~(srf::kTcFlagSplit | srf::kTcFlagPreproj);
+  if (precision == SRF_PREC_FP32_TC) f |= srf::kTcFlagSplit;
+  pp = p;
+  pp.preproj = (w.d_out == 4) ? p.preproj : p.preproj_gauss;
+  if (pp.preproj) f |= srf::kTcFlagPreproj;
+  return f;
+}
+
 int run_mlp(const srf::DevParams& p, int precision, int flags, const srf_mlp_weights& w, const float* pts,
             const float* viewdir, int n, int n_per, float* raw, int32_t* dbg, void* ws, size_t ws_bytes,
             cudaStream_t st, void* saved = nullptr) {
@@ -178,12 +189,8 @@ int run_mlp(const srf::DevParams& p, int precision, int flags, const srf_mlp_wei
     const srf::MatmulEngine e = saved ? matmul_engine(flags) : srf::MatmulEngine::simt;
     l = srf::run_point_mlp_simt(p, w, pts, viewdir, n, n_per, raw, dbg, saved, e, ws, ws_bytes, st);
   } else {
-    int f = flags & ~(srf::kTcFlagSplit | srf::kTcFlagPreproj);
-    if (precision == SRF_PREC_FP32_TC) f |= srf::kTcFlagSplit;
-    // a latent table belongs to one network: the main pass (d_out 4) reads latent_table, the proposal pass latent_table_gauss
-    srf::DevParams pp = p;
-    pp.preproj = (w.d_out == 4) ? p.preproj : p.preproj_gauss;
-    if (pp.preproj) f |= srf::kTcFlagPreproj;
+    srf::DevParams pp;
+    const int f = tc_pass(p, precision, flags, w, pp);
     l = srf::run_point_mlp_tc(pp, w, pts, viewdir, n, n_per, raw, dbg, f, ws, ws_bytes, st);
   }
   if (l < 0) return fail(SRF_E_WORKSPACE, "point-MLP workspace too small (%zu bytes)", ws_bytes);
@@ -851,9 +858,10 @@ int srf_debug_tc_layer(const srf_config* cfg, const srf_pyramid* pyr, const srf_
   const int d_latent = pyramid_channels(pyr);
   const bool split = cfg->precision == SRF_PREC_FP32_TC;
   if (int rc = validate_weights(w, w->d_out, d_latent, split ? SRF_PREC_FP32_TC : SRF_PREC_FP16_TC)) return rc;
-  const srf::DevParams p = make_params(cfg, pyr);
-  const int l = srf::run_point_mlp_tc_debug(p, *w, cam_pts_dev, viewdir_dev, n_cols * n_per, n_per, nullptr, nullptr,
-                                            split ? (cfg->flags | srf::kTcFlagSplit) : (cfg->flags & ~srf::kTcFlagSplit),
+  // the same pass as srf_predict's: this network's latent table when the pyramid carries one
+  srf::DevParams pp;
+  const int f = tc_pass(make_params(cfg, pyr), cfg->precision, cfg->flags, *w, pp);
+  const int l = srf::run_point_mlp_tc_debug(pp, *w, cam_pts_dev, viewdir_dev, n_cols * n_per, n_per, nullptr, nullptr, f,
                                             workspace_dev, workspace_bytes, layer, acc_out_dev, (cudaStream_t)stream);
   if (l == -1) return fail(SRF_E_WORKSPACE, "srf_debug_tc_layer: workspace too small");
   if (l < 0) return fail(SRF_E_INVALID, "srf_debug_tc_layer: layer %d has no accumulator-complete point", layer);

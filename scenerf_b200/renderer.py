@@ -404,9 +404,12 @@ class B200Renderer:
         _lib.check(self.lib.srf_last_mlp_ms(C.byref(g), C.byref(m)))
         return g.value, m.value
 
-    def debug_tc_layer(self, mlp, cam_pts, x_rgb, cam_K, viewdir, layer: int):
-        """Diagnostic: raw fp32 accumulator (ceil(n/tile)*64, 512; tile = 64 points, 32 in fp32tc) after `layer` of the tensor-core tile
-        program (include/scenerf_b200.h: srf_debug_tc_layer)."""
+    def debug_tc_layer(self, mlp, cam_pts, x_rgb, cam_K, viewdir, layer: int, out: Optional[torch.Tensor] = None):
+        """Diagnostic: raw fp32 accumulator after `layer` of the tensor-core tile program (include/scenerf_b200.h:
+        srf_debug_tc_layer), the same pass `predict` runs (latent-table variant included).  Tiles hold 64 points in
+        both modes.  fp16: (ceil(n/64)*64, 512), point i at row i.  fp32tc: (ceil(n/32)*64, 512), point i at row
+        64 (i//32) + i%32, in units of the weight scale 2^s.  Rows the kernel does not write keep the contents of
+        `out` (a float32 tensor of that shape on the renderer's device; zeros when omitted)."""
         net = self._select(mlp)
         if net.packed is None and net.packed_split is None:
             raise RuntimeError("renderer was not built with precision='fp16' / 'fp32tc'")
@@ -416,8 +419,13 @@ class B200Renderer:
         cfg = self._config(cam_K, None)
         pyr = self._pack_pyramid(x_rgb, cfg)
         n = n_cols * n_per
-        tile = 32 if self.precision == "fp32tc" else 64
-        acc = torch.zeros(((n + tile - 1) // tile * 64, 512), dtype=torch.float32, device=self.device)
+        rows = (n + 31) // 32 * 64 if self.precision == "fp32tc" else (n + 63) // 64 * 64
+        if out is None:
+            acc = torch.zeros((rows, 512), dtype=torch.float32, device=self.device)
+        else:
+            if out.dtype != torch.float32 or tuple(out.shape) != (rows, 512) or out.device != self.device or not out.is_contiguous():
+                raise ValueError("out must be a contiguous float32 (%d, 512) tensor on %s" % (rows, self.device))
+            acc = out
         ws = self._workspace(self.lib.srf_predict_workspace_bytes(C.byref(cfg), n))
         _lib.check(self.lib.srf_debug_tc_layer(C.byref(cfg), C.byref(pyr), C.byref(net.struct), _ptr(pts), _ptr(vd),
                                                n_cols, n_per, int(layer), _ptr(acc), _ptr(ws), ws.numel(),

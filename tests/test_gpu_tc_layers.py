@@ -1,85 +1,47 @@
-"""GPU: the wgmma tile program checked layer by layer.  After each accumulator-complete point of the fused kernel
-the raw fp32 accumulator is dumped (srf_debug_tc_layer) and compared with a float64 emulation that applies the
-same fp16 operand rounding (oracle geometry / gather / positional encoding + numpy matmuls).  This localises a wrong
-shared-memory descriptor, swizzle, weight image or epilogue to the exact layer."""
+"""GPU: the fp16 wgmma tile program (csrc/mlp_tc.cu, precision "fp16") checked entry by entry, layer by layer.
+
+After each accumulator-complete point of the fused kernel the raw fp32 accumulator is dumped (srf_debug_tc_layer) and
+every entry is compared with the chain-cut emulation of tests/tc_mlp_emul.py: the layer's A operand is rebuilt in
+float32 from the dumps of the layers before it, the reference and the bound ACC_C m_L 2^-24 sum|a||w| are float64.
+All four fp16 kernel variants (fp16 / fp32 hidden state, dense / latent table), both networks, shapes that hit the
+kernel's edges: the adversarial goldens, n = 1, n % 64 of 1 and 63, 13 and 1 points per view direction, and 2 SMs + 1
+tiles whose CTAs run tiles with different live lin_z chunks."""
 import numpy as np
 import pytest
 
-from cases import PREDICT_CASES, RENDER_CASES, load_golden, params_for, pyramid_for
+import tc_mlp_emul as E
+from cases import PREDICT_CASES, RENDER_CASES, load_golden
 from helpers import make_renderer, torch_pyramid
-from oracle import scenerf_oracle as orc
 
 pytestmark = pytest.mark.gpu
 
-
-def q16(a):
-    return np.asarray(a, dtype=np.float32).astype(np.float16).astype(np.float64)
+SHAPES = ("adv_kitti", "adv_bf", "n1", "n65_per13", "n127_per1", "multitile")
 
 
-def emulate(cfg, params, pts, viewdir, x_rgb):
-    """dict layer -> expected accumulator (n,512) with fp16-rounded operands, float64 accumulation."""
-    p = pts.reshape(-1, 3).astype(np.float32)
-    inv_K = np.linalg.inv(cfg.K).astype(np.float32)
-    coords, _ = orc.sphere_coords_from_pixels(orc.cam_pts_2_pix(p, cfg.K), inv_K, cfg.angles(), cfg.sphere_W, cfg.sphere_H)
-    # tensor-core mode stores the packed pyramid as fp16 (features rounded once at pack time)
-    x16 = {k: np.asarray(v, dtype=np.float32).astype(np.float16).astype(np.float32) for k, v in x_rgb.items()}
-    z = q16(orc.gather_latent(x16, coords, cfg.sphere_W, cfg.sphere_H))
-    x = q16(np.concatenate([orc.positional_encoding(p), np.repeat(viewdir, pts.shape[1], axis=0)], axis=1))
-    W = lambda n: q16(params[n])
-    b = lambda n: params[n].astype(np.float64)
-    out = {}
-    acc = x @ W("lin_in.weight").T + z @ W("lin_z.0.weight").T
-    out[1] = acc
-    h = acc + b("lin_in.bias") + b("lin_z.0.bias")
-    for blk in range(3):
-        # default tensor-core mode (SRF_FLAG_HIDDEN_FP16): the residual hidden state is stored as fp16 between blocks;
-        # the activation fed to fc_0 is relu(h) rounded to fp16, identical with or without that storage rounding
-        h_act = h
-        h = q16(h)
-        acc = q16(np.maximum(h_act, 0)) @ W("blocks.%d.fc_0.weight" % blk).T
-        out[2 + 3 * blk] = acc
-        net = acc + b("blocks.%d.fc_0.bias" % blk)
-        acc = q16(np.maximum(net, 0)) @ W("blocks.%d.fc_1.weight" % blk).T
-        if blk < 2:
-            acc = acc + z @ W("lin_z.%d.weight" % (blk + 1)).T
-            out[4 + 3 * blk] = acc
-            h = h + acc + b("blocks.%d.fc_1.bias" % blk) + b("lin_z.%d.bias" % (blk + 1))
-        else:
-            out[9] = acc
-            h = h + acc + b("blocks.%d.fc_1.bias" % blk)
-    o = q16(np.maximum(h, 0)) @ W("lin_out.weight").T
-    out[10] = o
-    out["final"] = o + b("lin_out.bias")
-    return out
-
-
-@pytest.mark.parametrize("which", ["mlp", "mlp_gaussian"])
-def test_tile_program_layer_by_layer(which):
+def _sms():
     import torch
-    cfg, seed = PREDICT_CASES["predict_adversarial_kitti"]
-    g = load_golden("predict_adversarial_kitti")
-    pts, vd = g["cam_pts"][:41], g["viewdir"][:41]        # 41 x 8 = 328 points: 6 tiles of 64, last one ragged
-    pm, pg = params_for(cfg)
-    params = pm if which == "mlp" else pg
-    exp = emulate(cfg, params, pts, vd, pyramid_for(cfg, seed))
-    r = make_renderer(cfg, "fp16")
-    x_rgb = torch_pyramid(cfg, seed)
-    K = torch.from_numpy(cfg.K)
-    n = pts.shape[0] * pts.shape[1]
-    for layer in (1, 2, 4, 5, 7, 8, 9, 10):
-        acc = r.debug_tc_layer(which, torch.from_numpy(pts), x_rgb, K, torch.from_numpy(vd), layer)
-        torch.cuda.synchronize()
-        got = acc.cpu().numpy()[:n]
-        want = exp[layer]
-        ncol = want.shape[1]
-        scale = float(np.abs(want).max())
-        err = float(np.abs(got[:, :ncol] - want).max())
-        print("%s layer %2d: max|acc| %.3e  max-abs-err %.3e" % (which, layer, scale, err))
-        assert err <= 2e-3 * scale + 1e-4, "layer %d: err %.3e (scale %.3e)" % (layer, err, scale)
-    raw = r.predict(which, torch.from_numpy(pts), x_rgb, K, None, torch.from_numpy(vd), output_type="offset")
-    got = raw.reshape(n, -1).cpu().numpy()
-    want = exp["final"]
-    assert np.abs(got - want).max() <= 2e-3 * np.abs(want).max() + 1e-4
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+@pytest.mark.parametrize("shape", SHAPES)
+@pytest.mark.parametrize("which", ["mlp", "mlp_gaussian"])
+@pytest.mark.parametrize("h16,table", [(True, False), (False, False), (True, True), (False, True)],
+                         ids=["h16", "h32", "h16-table", "h32-table"])
+def test_tile_program_per_entry(h16, table, which, shape):
+    cfg, seed, pts, vd = E.shape_case(shape, _sms())
+    E.check_variant(cfg, seed, "fp16", which, pts, vd, h16=h16, pre=table, label=shape)
+
+
+def test_skip_zero_chunks_multitile_per_entry_and_bit_identical():
+    """2 SMs + 1 tiles with different live lin_z chunks per tile: with and without zero-chunk skipping both pass the
+    per-entry check, and every dump and the output are bit-identical."""
+    import torch
+    cfg, seed, pts, vd = E.shape_case("multitile", _sms())
+    _, d0, r0 = E.check_variant(cfg, seed, "fp16", "mlp", pts, vd, skip=False, label="multitile")
+    _, d1, r1 = E.check_variant(cfg, seed, "fp16", "mlp", pts, vd, skip=True, label="multitile")
+    for L in E.LAYERS:
+        assert torch.equal(d0[L].view(torch.int32), d1[L].view(torch.int32)), L
+    assert torch.equal(r0, r1)
 
 
 def test_fp16_vs_fp32_device_paths_large_ragged():
